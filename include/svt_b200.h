@@ -1,5 +1,5 @@
 /*
- * svt_b200.h -- C ABI of libsvtav1_b200.so: the B200 (sm_100a) tier of SVT-AV1-PSY's inner-loop DSP.
+ * svt_b200.h -- C ABI of libsvtav1_b200.so: the H100 (sm_90a) tier of SVT-AV1-PSY's inner-loop DSP.
  *
  * Two layers (SURVEY.md F12):
  *
@@ -17,7 +17,7 @@
  *      "_host" variants take host buffers (copies are part of the call); "_dev" variants take
  *      device pointers + a CUDA stream (passed as void*) and only enqueue work.
  *
- * No CPU fallback exists: svt_b200_init() fails unless an sm_100 device is present and every other
+ * No CPU fallback exists: svt_b200_init() fails unless an sm_90 device is present and every other
  * entry point aborts if it has not succeeded.
  *
  * Types are plain C (stdint); no CUDA or torch types appear in any signature.
@@ -44,7 +44,7 @@ extern "C" {
 enum {
     SVT_B200_OK               = 0,
     SVT_B200_ERR_NO_DEVICE    = -1, /* maps to EB_ErrorInsufficientResources at svt_av1_enc_init time */
-    SVT_B200_ERR_BAD_ARCH     = -2, /* device is not sm_100 */
+    SVT_B200_ERR_BAD_ARCH     = -2, /* device is not sm_90 */
     SVT_B200_ERR_ALREADY_INIT = -3,
     SVT_B200_ERR_BAD_ARG      = -4
 };

@@ -13,7 +13,7 @@
 
 /* ---- adaptors where the reference's calling convention is not a plain pointer list ---------------------------------- */
 /* svt_av1_inv_txfm_add (common_dsp_rtcd.h:144): the 8-bit inverse takes its transform type / size in a TxfmParam.
- * Lossless blocks use the Walsh-Hadamard transform, which is not on the B200 path: they stay on the C function. */
+ * Lossless blocks use the Walsh-Hadamard transform, which is not on the H100 path: they stay on the C function. */
 static void b200_av1_inv_txfm_add(const TranLow* dqcoeff, uint8_t* dst_r, int32_t stride_r, uint8_t* dst_w, int32_t stride_w,
                                   const TxfmParam* p) {
     if (p->lossless) {
@@ -23,7 +23,7 @@ static void b200_av1_inv_txfm_add(const TranLow* dqcoeff, uint8_t* dst_r, int32_
     svt_b200_inv_txfm_add_8bit(dqcoeff, dst_r, stride_r, dst_w, stride_w, (int)p->tx_type, (int)p->tx_size);
 }
 /* High-bit-depth pixel pointers travel through uint8_t* arguments as CONVERT_TO_BYTEPTR disguises (address >> 1:
- * full_loop.c:1843-1846, restoration.c:933); the B200 entry points take the real uint16_t address. */
+ * full_loop.c:1843-1846, restoration.c:933); the H100 entry points take the real uint16_t address. */
 #define B200_U16(p) ((const uint16_t*)CONVERT_TO_SHORTPTR(p))
 static void b200_highbd_wiener_convolve_add_src(const uint8_t* const src, const ptrdiff_t src_stride, uint8_t* const dst,
                                                 const ptrdiff_t dst_stride, const int16_t* const filter_x, const int16_t* const filter_y,
@@ -204,8 +204,8 @@ void svt_b200_setup_rtcd_then_install(uint64_t flags) {
     const char* dev = getenv("SVT_B200_DEVICE");
     if ((flags & EB_CPU_FLAGS_B200) || (dev && *dev)) {
         const int rc = svt_b200_install_rtcd(dev && *dev ? atoi(dev) : 0);
-        if (rc != 0) { /* no CPU fallback: an encoder asked to run on the B200 tier must not silently run on the host */
-            fprintf(stderr, "[svt_b200] FATAL: svt_b200_install_rtcd failed (%d): an sm_100 device is required\n", rc);
+        if (rc != 0) { /* no CPU fallback: an encoder asked to run on the H100 tier must not silently run on the host */
+            fprintf(stderr, "[svt_b200] FATAL: svt_b200_install_rtcd failed (%d): an sm_90 device is required\n", rc);
             abort();
         }
     }

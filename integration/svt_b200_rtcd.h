@@ -1,4 +1,4 @@
-/* svt_b200_rtcd.h -- the B200 tier's binding into SVT-AV1-PSY's run-time dispatch.
+/* svt_b200_rtcd.h -- the H100 tier's binding into SVT-AV1-PSY's run-time dispatch.
  *
  * A reference build adds integration/svt_b200_rtcd.c to Source/Lib/Globals and calls
  *     svt_b200_install_rtcd(device)

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY.  CPU checkers for the B200 DSP path:
+"""TEST INFRASTRUCTURE ONLY.  CPU checkers for the H100 DSP path:
 
   oracle.port  -- ctypes handle on oracle/_ref/liboracle_port.so, our C restatement (oracle/port/*.c)
   oracle.ref   -- ctypes handle on oracle/_ref/libsvtav1_ref.so, the UNMODIFIED reference sources

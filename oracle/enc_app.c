@@ -2,7 +2,7 @@
  * (Source/API/EbSvtAv1Enc.h; the call sequence of Source/App/app_process_cmd.c:577-590,866-935, restated): encodes
  * raw planar 4:2:0 frames held in memory and returns the concatenated OBU packets.  Compiled into
  * oracle/_ref/libsvtav1_enc.so next to the UNMODIFIED reference library sources; with the environment variable
- * SVT_B200_DEVICE set, the rtcd hook (integration/svt_b200_rtcd.c) installs the B200 tier at enc_handle.c:1445, so
+ * SVT_B200_DEVICE set, the rtcd hook (integration/svt_b200_rtcd.c) installs the H100 tier at enc_handle.c:1445, so
  * the same call encodes once on the C path and once with every hot-path DSP pointer served by libsvtav1_b200.so --
  * the bitstreams must be identical (SURVEY.md 8(c)(ii)). */
 #include <stdint.h>

@@ -20,7 +20,7 @@ vp = ct.c_void_p
 
 def load_workload_module():
     """svt-av1-psy_b200/workload.py + layout.py as top-level modules (no package __init__, no .so)"""
-    if "svt_av1_psy_b200.workload" in sys.modules:  # the product package is already imported (tests, B200 arm)
+    if "svt_av1_psy_b200.workload" in sys.modules:  # the product package is already imported (tests, H100 arm)
         return sys.modules["svt_av1_psy_b200.workload"]
     if _PKG not in sys.path:
         sys.path.append(_PKG)

@@ -1,7 +1,7 @@
 /* oracle/ref_driver.c -- TEST / BASELINE INFRASTRUCTURE, compiled INTO oracle/_ref/libsvtav1_ref.so.
  *
  * Whole-picture drivers that run the UNMODIFIED reference kernels (through the reference's own
- * dispatch pointers) over the same work lists the B200 T2 entry points take, so that
+ * dispatch pointers) over the same work lists the H100 T2 entry points take, so that
  *   (1) the T2 paths can be checked against the reference at picture scale, and
  *   (2) bench.py --impl reference / cpu_baseline can time the reference's CPU path (C tier, or the
  *       intrinsics-only AVX2 tier) on all host cores (OpenMP) for the same workload.
@@ -213,7 +213,7 @@ int ref_set_tier(int avx2) {
 /* ---- open-loop ME for one picture ---------------------------------------------------------------
  * restates hme_level_0/1/2 (motion_estimation.c:820-1113), set_final_seach_centre_sb (:2182-2390),
  * check_00_center (:1139-1210), integer_search_b64 (:1249-1520), open_loop_me_fullpel_search_sblock
- * (:781-817) for the controls the B200 T2 path honours (see DESIGN.md). */
+ * (:781-817) for the controls the H100 T2 path honours (see DESIGN.md). */
 #include "ref_me_b64.h" /* RefMePicture + the complete driver (ref_me_b64.c) */
 typedef struct { int32_t hme_l0_sa_w, hme_l0_sa_h, hme_l1_sa_w, hme_l1_sa_h, hme_l2_sa_w, hme_l2_sa_h, me_sa_w, me_sa_h, hme_sub_sad, me_sub_sad, check_zero_centre, reserved; } RefMeParams;
 

@@ -6,7 +6,7 @@
  * full-pel search / candidate construction / distortion for every 64x64 block -- none of that control flow is
  * restated here.  What this file does is what the encoder's picture-level processes do around that call
  * (me_process.c:120-270): allocate a PictureParentControlSet / SequenceControlSet / MeContext, point them at the
- * caller's picture pyramids, and copy the results out.  The B200 T2 call svt_b200_me_b64_picture_dev is checked
+ * caller's picture pyramids, and copy the results out.  The H100 T2 call svt_b200_me_b64_picture_dev is checked
  * against these outputs (tests/test_me_b64.py), and bench.py's reference arm times this function.
  * Nothing here is used by the product. */
 #include <stdint.h>

@@ -1,4 +1,4 @@
-"""svt-av1-psy_b200: B200 (sm_100a) tier of SVT-AV1-PSY's inner-loop DSP.
+"""svt-av1-psy_b200: H100 (sm_90a) tier of SVT-AV1-PSY's inner-loop DSP.
 
 The product is `libsvtav1_b200.so` (hand-written CUDA behind a C ABI, include/svt_b200.h).  This
 package is the thin host-side mirror used by tests and bench: it loads the library with ctypes,
@@ -6,7 +6,7 @@ verifies that every symbol the header declares is exported, and exposes numpy-le
 carry the reference's function names (Source/Lib/Codec/aom_dsp_rtcd.h, common_dsp_rtcd.h).
 
 There is no CPU fallback: importing works without a GPU (symbol check only), but any compute call
-requires `init()` to have bound an sm_100 device and aborts otherwise.
+requires `init()` to have bound an sm_90 device and aborts otherwise.
 """
 import ctypes as _ct
 import os as _os
@@ -19,7 +19,7 @@ HEADER_PATH = _os.path.join(_os.path.dirname(_PKG_DIR), "include", "svt_b200.h")
 
 if not _os.path.exists(LIB_PATH):
     raise ImportError(
-        "libsvtav1_b200.so is missing (%s). Run `python __graft_entry__.py` (nvcc, sm_100a) first; "
+        "libsvtav1_b200.so is missing (%s). Run `python __graft_entry__.py` (nvcc, sm_90a) first; "
         "this package has no CPU fallback." % LIB_PATH)
 
 lib = _ct.CDLL(LIB_PATH)

@@ -1,5 +1,5 @@
 // cdef.cu -- K8 CDEF: direction search, constrained directional filter, distortion, strength search,
-// frame apply (sm_100a).
+// frame apply (sm_90a).
 //
 // Reference behaviour restated: svt_aom_cdef_find_dir_c (Source/Lib/Codec/cdef.c:150-210),
 // constrain/adjust_strength (:85-134), svt_cdef_filter_block_c (:253-305), svt_cdef_filter_fb (:339-430),
@@ -7,7 +7,7 @@
 // svt_search_one_dual_c (:627-690), the tile build of cdef_seg_search (Source/Lib/Codec/cdef_process.c:
 // 106-352: CDEF_VERY_LARGE outside the frame, pre-filter neighbours inside).
 //
-// B200 mapping (T2): a frame-wide kernel finds direction and variance of every non-skip 8x8 (one
+// H100 mapping (T2): a frame-wide kernel finds direction and variance of every non-skip 8x8 (one
 // thread per block, the 64 pixels in registers).  Search and apply run one CTA per (64x64 filter block,
 // plane): the padded 16-bit tile of the plane is staged in shared memory once and every filtered pixel
 // is one thread.  A pixel's 12 taps are fetched once per direction, as signed differences and magnitudes

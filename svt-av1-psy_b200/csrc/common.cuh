@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device plumbing for libsvtav1_b200.so (sm_100a only).
+// common.cuh -- shared host/device plumbing for libsvtav1_b200.so (sm_90a only).
 //
 // The library mirrors the reference's process-global dispatch model
 // (Source/Lib/Codec/aom_dsp_rtcd.c:188, common_dsp_rtcd.c:466): one global context, entry points

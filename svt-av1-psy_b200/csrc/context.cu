@@ -96,8 +96,8 @@ extern "C" int svt_b200_init(int device) {
     if (device >= n) return SVT_B200_ERR_NO_DEVICE;
     cudaDeviceProp p;
     if (cudaGetDeviceProperties(&p, device) != cudaSuccess) return SVT_B200_ERR_NO_DEVICE;
-    if (p.major != 10) {
-        fprintf(stderr, "[svt_b200] device %d is sm_%d%d; this library is built for sm_100a only\n", device, p.major,
+    if (p.major != 9) {
+        fprintf(stderr, "[svt_b200] device %d is sm_%d%d; this library is built for sm_90a only\n", device, p.major,
                 p.minor);
         return SVT_B200_ERR_BAD_ARCH;
     }
@@ -156,7 +156,7 @@ extern "C" int svt_b200_copy2d_async(void* dst, size_t dst_pitch, const void* sr
 
 extern "C" int svt_b200_sm_count(void) { return ctx().ready ? ctx().sm_count : 0; }
 extern "C" unsigned long long svt_b200_launch_count(void) { return ctx().launches; }
-extern "C" const char* svt_b200_version(void) { return "svt_b200 0.1 (sm_100a)"; }
+extern "C" const char* svt_b200_version(void) { return "svt_b200 0.1 (sm_90a)"; }
 
 namespace b200 {
 

@@ -1,4 +1,4 @@
-// hadamard.cu -- K4 Hadamard transforms and SATD (sm_100a).
+// hadamard.cu -- K4 Hadamard transforms and SATD (sm_90a).
 //
 // Reference behaviour restated: svt_aom_hadamard_{4x4,8x8,16x16,32x32}_c
 // (Source/Lib/C_DEFAULT/picture_operators_c.c:188-330: 1-D butterflies on int16 with wrap, >>1 inside

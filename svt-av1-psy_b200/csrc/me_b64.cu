@@ -1,4 +1,4 @@
-// me_b64.cu -- T2, the COMPLETE open-loop ME driver of a picture (sm_100a): everything svt_aom_motion_estimation_b64 does for
+// me_b64.cu -- T2, the COMPLETE open-loop ME driver of a picture (sm_90a): everything svt_aom_motion_estimation_b64 does for
 // a 64x64 block, for all blocks and all reference pictures, in three launches.
 //
 // Reference behaviour restated (Source/Lib/Codec/motion_estimation.c):
@@ -16,7 +16,7 @@
 //   perform_gm_detection            :2842
 //
 // Launches:  (A) me_b64_hme_kernel<PAR>  one CTA per 64x64 block, 4 * PAR warps.  The references are walked in the reference's
-//                order, PAR at a time (1, or 2 from six references up: measured); inside the HME stages a warp is one
+//                order, PAR at a time (1, or 2 from six references up: chosen on the previous target GPU, not re-measured on H100); inside the HME stages a warp is one
 //                (reference, search region) pair, in the per-reference stages (zz SAD, pre-HME, window derivation) one reference.
 //                Decisions that couple references (pruning, carried-over centres) are taken by one thread between barriers.
 //                Writes one full-pel item per (reference, block) + the 85 SADs of the variance probe ("seed").
@@ -85,7 +85,10 @@ __device__ __forceinline__ uint32_t warp_sad_every_other_row(const uint8_t* src,
 // the 85 SADs of ONE search position (src block vs ref block, both 64x64), written in the ME's PU order
 // (64x64, 4 x 32x32, 16 x 16x16 and 64 x 8x8 in z order) -- what open_loop_me_fullpel_search_sblock(..., 1, 1) leaves in
 // p_sb_best_sad.  lane handles the 8x8 blocks 2*lane and 2*lane+1 (z order), sub = rows 0,2,4,6 only, doubled.
-__device__ __forceinline__ void warp_probe_sads(const uint8_t* src, int ss, const uint8_t* ref, int rs, bool sub, int lane, uint32_t* out85) {
+// Returns, in every lane, the variance of the 64 8x8 SADs about their mean (sum / 64 of the squared deviations, 32-bit
+// arithmetic as in the reference).  It is computed from registers: out85 is only for the search kernel that runs next, and
+// a lane must not read another lane's stores there (the compiler may move such a load above the warp barrier).
+__device__ __forceinline__ uint32_t warp_probe_sads(const uint8_t* src, int ss, const uint8_t* ref, int rs, bool sub, int lane, uint32_t* out85) {
     uint32_t s8[2];
 #pragma unroll
     for (int k = 0; k < 2; k++) {
@@ -111,6 +114,9 @@ __device__ __forceinline__ void warp_probe_sads(const uint8_t* src, int ss, cons
     if ((lane & 1) == 0) out85[5 + (lane >> 1)] = v16;
     if ((lane & 7) == 0) out85[1 + (lane >> 3)] = v32;
     if (lane == 0) out85[0] = v64;
+    const uint32_t mean = v64 / 64u;
+    const int32_t  d0 = (int32_t)s8[0] - (int32_t)mean, d1 = (int32_t)s8[1] - (int32_t)mean;
+    return __reduce_add_sync(0xffffffffu, (uint32_t)(d0 * d0) + (uint32_t)(d1 * d1)) / 64u;
 }
 
 // integer_search_b64's clipping of the search window (same arithmetic as the HME levels, against the ALIGNED picture size)
@@ -517,17 +523,8 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
         }
         // 8x8-SAD-variance probe at the search centre
         if (c.var_enable && (int)sa_w * (int)sa_h > 24) {
-            uint32_t* seed = seed_sad + item_idx * 85;
-            warp_probe_sads(src_full, cur.stride[2], r0 + (ptrdiff_t)sy * rp.stride[2] + sx, rp.stride[2], c.me_sub_sad != 0, lane, seed);
-            __syncwarp();
-            const uint32_t mean = seed[0] / 64u;
-            uint32_t       sq = 0;
-            for (int k = lane; k < 64; k += 32) {
-                const int32_t d = (int32_t)seed[21 + k] - (int32_t)mean;
-                sq += (uint32_t)(d * d);
-            }
-            sq = __reduce_add_sync(0xffffffffu, sq);
-            const uint32_t var = sq / 64u;
+            const uint32_t var = warp_probe_sads(src_full, cur.stride[2], r0 + (ptrdiff_t)sy * rp.stride[2] + sx, rp.stride[2], c.me_sub_sad != 0,
+                                                 lane, seed_sad + item_idx * 85);
             if (var > (uint32_t)c.var_mult2_th) {
                 sa_w = (int16_t)((max(1, sa_w * 3 / 2) + 7) & ~0x7);
                 sa_h = (int16_t)max(1, sa_h * 3 / 2);
@@ -822,8 +819,8 @@ extern "C" int svt_b200_me_b64_picture_dev(const SvtB200MePicture* cur, const Sv
     B200_CUDA_CHECK(cudaMemsetAsync(out->total_me_candidate_index, 0, (size_t)n_b64 * n_pu, st));
     B200_CUDA_CHECK(cudaMemsetAsync(out->me_candidate_array, 0, (size_t)n_b64 * n_pu * c.max_cand, st));
     B200_CUDA_CHECK(cudaMemsetAsync(out->me_mv_array, 0, (size_t)n_b64 * n_pu * c.max_refs * 4, st));
-    // two references of a block in flight per CTA pays off with many references (measured: 7 references at 2160p M4, ME call
-    // 1.025 -> 0.954 ms) and costs with few (4 references at 1080p M8: 0.125 -> 0.156 ms): profiles/README.md
+    // two references of a block in flight per CTA pays off with many references and costs with few (chosen on the previous target
+    // GPU; not re-measured on H100)
     if (n_refs >= 6)
         me_b64_hme_kernel<2><<<n_b64, 256, 0, st>>>(tab, n_b64, b64_w, w->items, w->seed, w->do_ref, out->hme_centre, out->zz_sad);
     else

@@ -1,5 +1,5 @@
 // me_picture.cu -- T2 open-loop motion estimation for a whole picture: HME pyramid construction (K13),
-// HME level 0/1/2, final search centre, zero-centre check and the 85-PU full-pel search (sm_100a).
+// HME level 0/1/2, final search centre, zero-centre check and the 85-PU full-pel search (sm_90a).
 //
 // Reference behaviour restated (the "core" open-loop path; see DESIGN.md for the MeContext controls
 // that are honoured and those that are not):

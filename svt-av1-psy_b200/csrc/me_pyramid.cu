@@ -1,5 +1,5 @@
 // me_pyramid.cu -- K2 SAD pyramid (8x8 -> 16x16 -> 32x32 -> 64x64) and the T2 full-pel search that
-// is built from it (sm_100a).
+// is built from it (sm_90a).
 //
 // Reference behaviour restated:
 //   svt_ext_all_sad_calculation_8x8_16x16_c   Source/Lib/Codec/motion_estimation.c:335-363 (+:210-333)
@@ -168,7 +168,7 @@ __device__ __forceinline__ void stage_rows(uint32_t* dst, int nwords, int rows, 
     }
 }
 
-// ---- TMA plumbing (sm_100a): one elected thread arms an mbarrier with the byte count and issues cp.async.bulk.tensor;
+// ---- TMA plumbing (sm_90a): one elected thread arms an mbarrier with the byte count and issues cp.async.bulk.tensor;
 // the box lands in shared memory with no per-thread address arithmetic, alignment fix-up or funnel shifts --------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
@@ -189,9 +189,9 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
 }
 
 constexpr int kFpTmaRefs = 8;                     // reference pictures per launch that can be addressed through tensor maps
-// A box must START on a 16-byte boundary of global memory (measured on this GPU with tools/probe/tma_probe.cu: any other
-// innermost coordinate of a 1-byte tensor raises "illegal instruction"), a search window starts anywhere: the box is taken from
-// the aligned address below it, 16 bytes wider, and the positions are addressed with the residual byte offset.
+// Design rule: every box of a 1-byte tensor starts on a 16-byte aligned innermost coordinate.  A search window starts anywhere,
+// so its box is taken from the aligned address below it, 16 bytes wider, and the positions are addressed with the residual
+// byte offset.
 constexpr int kFpBoxW = 96, kFpBoxH = kFpLines;   // bytes x rows of one window box (15 + kFpTW + 63 = 94 bytes used)
 constexpr int kFpSrcBoxW = 80;                    // source block: 64 bytes + up to 12 of alignment slack (word-aligned origins only)
 struct FpTma {
@@ -524,7 +524,7 @@ extern "C" void svt_b200_ext_sad_calculation_8x8_16x16(uint8_t* src, uint32_t sr
 }
 
 // svt_initialize_buffer_32bits (aom_dsp_rtcd.h:855): pure host-memory fill; there is nothing for a
-// device to do here, so the B200 tier keeps it as the trivial host loop it is.
+// device to do here, so the H100 tier keeps it as the trivial host loop it is.
 extern "C" void svt_b200_initialize_buffer_32bits(uint32_t* pointer, uint32_t count128, uint32_t count32, uint32_t value) {
     const uint32_t n = count128 * 4 + count32;
     for (uint32_t i = 0; i < n; i++) pointer[i] = value;

@@ -1,4 +1,4 @@
-// quant.cu -- K7 quantize / dequantize (sm_100a).
+// quant.cu -- K7 quantize / dequantize (sm_90a).
 //
 // Reference behaviour restated: svt_aom_quantize_b_c_ii (Source/Lib/Codec/full_loop.c:29-79),
 // svt_aom_highbd_quantize_b_c (:149-198), quantize_fp_helper_c (:282-342), highbd_quantize_fp_helper_c

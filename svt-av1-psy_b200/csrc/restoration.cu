@@ -1,4 +1,4 @@
-// restoration.cu -- a13: loop-restoration drivers on the device (sm_100a).
+// restoration.cu -- a13: loop-restoration drivers on the device (sm_90a).
 //
 // Reference behaviour restated (Source/Lib/Codec/restoration.c):
 //   svt_av1_loop_restoration_save_boundary_lines (:1682) / svt_aom_save_tile_row_boundary_lines (:1606) /
@@ -12,7 +12,7 @@
 //   <= 64-wide column chunks; RESTORE_NONE units are copied;
 //   sse_restoration_unit (restoration_pick.c:103): squared error of a unit against the source (the trial cost of the RU search).
 //
-// B200 mapping.  The reference patches the picture rows in place around every stripe and restores them afterwards -- a
+// H100 mapping.  The reference patches the picture rows in place around every stripe and restores them afterwards -- a
 // serial save / overwrite / filter / restore dance.  Here one CTA owns one (stripe, 64-column chunk) of a plane: it
 // stages the (h + 7) x (w + 8) input tile into shared memory, fetching each halo row from wherever the reference would
 // have found it (picture, saved above / below line, or the neighbouring picture row in optimized_lr mode), looks up the

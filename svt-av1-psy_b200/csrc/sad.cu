@@ -1,11 +1,11 @@
-// sad.cu -- K1 full-search SAD (svt_sad_loop_kernel) and K3 single SAD, sm_100a.
+// sad.cu -- K1 full-search SAD (svt_sad_loop_kernel) and K3 single SAD, sm_90a.
 //
 // Reference behaviour restated (not translated): Source/Lib/C_DEFAULT/compute_sad_c.c:58-101.
 //   for y in [0,sa_h): (optionally skip even y when bw==16 && bh<=16 && skip_search_line)
 //     for x in [0,sa_w):  sad(x,y) = sum |src[r*src_stride+c] - ref[y*ref_step + x + r*ref_stride + c]|
 //     strict '<' update  => the FIRST minimum in raster order wins.
 //
-// B200 design.  Searches of at most 256 positions (every HME / ME refinement of the presets in scope) take
+// H100 design.  Searches of at most 256 positions (every HME / ME refinement of the presets in scope) take
 // the warp-per-search path of sad_small.cuh; larger areas the tiled kernel below: one CTA per work item
 // (grid-stride over the list, so one launch serves a whole picture's searches).  The block and a tile of the search window are staged in shared memory as
 // 32-bit words; a thread owns M search positions x, x+4, ... x+4(M-1) of one search row so that the

@@ -111,8 +111,8 @@ __device__ __forceinline__ unsigned long long sad_search_warp_w16(const uint8_t*
                 }
             }
         }
-        // Sum the 8 position accumulators over the lanes of the group.  Shuffle trees, not REDUX (__reduce_add_sync): measured on
-        // this GPU the one-instruction form costs several times a SHFL + IADD pair (profiles/README.md, CDEF search experiment).
+        // Sum the 8 position accumulators over the lanes of the group.  Shuffle trees, not REDUX (__reduce_add_sync): chosen by
+        // kernel times taken on the previous target GPU (not re-measured on H100).
         // Lane distances >= 8 are plain butterflies; the last three steps halve the number of live accumulators each time
         // (a lane keeps the half selected by its own lane bit and hands the other half over), so lane L ends up with the total of
         // position L & 7: 7 shuffles instead of 24.

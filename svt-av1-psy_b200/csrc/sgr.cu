@@ -1,4 +1,4 @@
-// sgr.cu -- K10 self-guided restoration filter, K12 projection error / projection subspace (sm_100a).
+// sgr.cu -- K10 self-guided restoration filter, K12 projection error / projection subspace (sm_90a).
 //
 // Reference behaviour restated:
 //   svt_av1_selfguided_restoration_c (Source/Lib/Codec/restoration.c:923-955) with

@@ -1,11 +1,11 @@
-// txfm.cu -- K5 forward 2-D transforms, K6 inverse 2-D transforms + reconstruction (sm_100a).
+// txfm.cu -- K5 forward 2-D transforms, K6 inverse 2-D transforms + reconstruction (sm_90a).
 //
 // Reference behaviour restated: av1_tranform_two_d_core_c (Source/Lib/Codec/transforms.c:2259-2324)
 // and inv_txfm2d_add_c (Source/Lib/Codec/inv_transforms.c:2459-2534), for all 19 transform sizes and
 // 16 transform types, 8/10/12-bit.  The 2-D configuration table (flips, per-pass kernel, cos_bit,
 // shifts) is dumped from the reference (txfm_cfg.inc); the 1-D networks are txfm_graphs.inc.
 //
-// B200 mapping: a team of max(W,H) threads per transform block (4, 8, 16, 32 or 64: the block's
+// H100 mapping: a team of max(W,H) threads per transform block (4, 8, 16, 32 or 64: the block's
 // "team class"), one thread per column in the column pass and one per row in the row pass, each
 // running the generated straight-line network on its vector in registers (txfm_tables.cuh).  The
 // block sits in shared memory in element-major order with an odd pitch, so the passes and the

@@ -1,4 +1,4 @@
-// wiener.cu -- K9 separable Wiener filter, K11 Wiener statistics (M = Y^T x, H = Y^T Y) (sm_100a).
+// wiener.cu -- K9 separable Wiener filter, K11 Wiener statistics (M = Y^T x, H = Y^T Y) (sm_90a).
 //
 // Reference behaviour restated:
 //   svt_av1_wiener_convolve_add_src_c / svt_av1_highbd_wiener_convolve_add_src_c
@@ -9,7 +9,7 @@
 //     per pixel the wiener_win^2 window of (dgd - avg) is the vector y (column-major), x = src - avg;
 //     M[k] += y[k] x, H[k][l] += y[k] y[l]; high bit depth divides by 4 / 16 at the end (truncating).
 //
-// B200 mapping of the statistics (the one dense contraction on the path):
+// H100 mapping of the statistics (the one dense contraction on the path):
 //   8-bit pixels -> stats_mma_kernel: exact f16 x f16 -> f32 tensor-core MMA (see the comment above it);
 //   10/12-bit    -> the lag-sum kernels of wiener_stats_lag.cuh (H[p][q] depends only on the lag between the two samples).
 // The MMA kernel writes per-CTA int64 partials; stats_finalize_kernel adds them, mirrors the triangle and applies

@@ -1,4 +1,4 @@
-// wiener_stats_lag.cuh -- K11 Wiener statistics by LAG sums (sm_100a), included by wiener.cu.
+// wiener_stats_lag.cuh -- K11 Wiener statistics by LAG sums (sm_90a), included by wiener.cu.
 //
 // Reference: svt_av1_compute_stats_c / _highbd_c (Source/Lib/Codec/restoration_pick.c:659-745).  With y_p(i,j) =
 // dgd(i + lr_p, j + kc_p) - avg the window sample p of pixel (i,j) (p = (kc + half) * win + (lr + half)) and x = src - avg,

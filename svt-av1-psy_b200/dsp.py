@@ -67,11 +67,11 @@ _initialised = False
 
 
 def init(device=0):
-    """Bind the library to a CUDA device (svt_b200_init).  Raises if no sm_100 device is usable."""
+    """Bind the library to a CUDA device (svt_b200_init).  Raises if no sm_90 device is usable."""
     global _initialised
     rc = lib.svt_b200_init(int(device))
     if rc != 0:
-        raise RuntimeError("svt_b200_init(%d) failed with %d: an sm_100 (B200) device is required; "
+        raise RuntimeError("svt_b200_init(%d) failed with %d: an sm_90 (H100) device is required; "
                            "there is no CPU fallback" % (device, rc))
     _initialised = True
     return rc

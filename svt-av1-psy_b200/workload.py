@@ -1,4 +1,4 @@
-"""Synthetic "1080p preset-8 hot path" workload: the per-frame work lists the B200 T2 entry points
+"""Synthetic "1080p preset-8 hot path" workload: the per-frame work lists the H100 T2 entry points
 (and, in bench.py's reference arm, the reference's own kernels) are driven with.
 
 One frame of work = what the reference's ME, EncDec (final encode pass), CDEF and REST process
@@ -154,6 +154,7 @@ class FrameWorkload:
         return planes[0] if self.bit_depth == 8 else (planes[0] >> (self.bit_depth - 8)).astype(np.uint8)
 
     def _set_pictures(self, seed):
+        self.seed = seed
         back, fwd = max(-d for d in ME_DIST[0][:self.n_ref[0]]), max((0,) + ME_DIST[1][:self.n_ref[1]])
         seq = synth_sequence(self.width, self.height, back + fwd + 1, seed, self.bit_depth)
         self.cur = seq[back]

@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
 def b200():
-    """The product library bound to cuda:0 (fails loudly when there is no sm_100 device)."""
+    """The product library bound to cuda:0 (fails loudly when there is no sm_90 device)."""
     import svt_av1_psy_b200 as pkg
     pkg.init(0)
     yield pkg.dsp
@@ -29,11 +29,11 @@ def oracle():
 
 @pytest.fixture(scope="session")
 def refc(oracle, request):
-    """ctypes handle on the unmodified reference objects.  On a GPU run (-m gpu) a missing oracle is an ERROR -- the
-    parity tests must not silently skip there; the CPU suite may run on a clone without /root/reference."""
+    """ctypes handle on the unmodified reference objects.  For a GPU test a missing oracle is an ERROR -- the parity
+    tests must not silently skip; the CPU pins may run on a clone where the reference sources are not available."""
     if oracle.ref is None:
-        if "gpu" in (request.config.getoption("-m") or ""):
+        if request.node.get_closest_marker("gpu") is not None:
             pytest.fail("oracle/_ref/libsvtav1_ref.so is missing: build it with `python __graft_entry__.py --oracle` where "
-                        "/root/reference exists (it travels to the GPU box with the repository)")
+                        "the reference sources are available")
         pytest.skip("oracle/_ref/libsvtav1_ref.so not built (no /root/reference)")
     return oracle.ref

@@ -1,6 +1,7 @@
-"""GPU parity at picture scale: one frame through the T2 pipeline (the path bench.py times) against
-the reference arm -- the reference's own kernels driven by oracle/ref_driver.c -- bit for bit, at a
-small size and at BASELINE's 1920x1080."""
+"""GPU parity at picture scale: one frame through the T2 pipeline (the path bench.py times), every output compared
+bit for bit with the committed SHA-256 digests of what the reference's own kernels compute for the same seeded frame
+(tests/golden/, tools/make_golden.py; pinned against the reference by tests/test_oracle_pins.py), at small sizes and at
+every BASELINE configuration."""
 import pytest
 
 pytestmark = pytest.mark.gpu
@@ -12,18 +13,19 @@ FRAME_CASES = [(384, 256, 8, 8), (384, 256, 10, 6), (448, 320, 10, 4), (1920, 10
 
 
 @pytest.mark.parametrize("case", FRAME_CASES, ids=lambda c: "%dx%d_b%d_m%d" % c)
-def test_frame_pipeline_matches_reference(b200, refc, case):
+def test_frame_pipeline_matches_reference(b200, case):
     """every output of the T2 frame pipeline == the reference's own kernels (8-bit: svt_av1_inv_txfm_add, svt_av1_compute_stats,
     svt_av1_wiener_convolve_add_src ...; 10-bit: svt_aom_inv_transform_recon with CONVERT_TO_BYTEPTR planes as in
     full_loop.c:1843-1846, svt_av1_highbd_quantize_fp_qm, svt_compute_cdef_dist_16bit, svt_av1_compute_stats_highbd,
-    svt_av1_highbd_wiener_convolve_add_src as in restoration.c:933)"""
+    svt_av1_highbd_wiener_convolve_add_src as in restoration.c:933), through the committed digests of the reference's
+    outputs (tests/golden/, pinned against the reference by test_oracle_pins.py)"""
     import torch
     import bench
     from svt_av1_psy_b200.pipeline import FramePipeline
     from svt_av1_psy_b200.workload import FrameWorkload
     w, h, bd, m = case
     fp = FramePipeline(FrameWorkload(w, h, bit_depth=bd, preset=m), torch)
-    bench.check_against_reference(fp, torch)
+    bench.check_against_golden(fp, torch)
     # size-independent property: a second pass over the same inputs is idempotent
     a = fp.final.clone(), fp.qcoeff.clone(), fp.me["me_mv_array"].clone()
     fp.step()
@@ -31,7 +33,7 @@ def test_frame_pipeline_matches_reference(b200, refc, case):
     assert torch.equal(a[0], fp.final) and torch.equal(a[1], fp.qcoeff) and torch.equal(a[2], fp.me["me_mv_array"])
 
 
-def test_cdef_apply_recomputes_directions_when_none_given(b200, refc):
+def test_cdef_apply_recomputes_directions_when_none_given(b200):
     """svt_b200_cdef_apply_frame_dev with d_dir = d_var = NULL finds the directions itself; the result
     must equal the apply that reuses the arrays of the search."""
     import ctypes as ct
@@ -57,7 +59,7 @@ def test_cdef_apply_recomputes_directions_when_none_given(b200, refc):
                                                  fp.app_uv.data_ptr(), fp.cdef_dir.data_ptr(), None, oy, ocb, ocr, sy, sc, s) == -4  # SVT_B200_ERR_BAD_ARG
 
 
-def test_two_frames_in_flight_on_two_streams(b200, refc):
+def test_two_frames_in_flight_on_two_streams(b200):
     """bench.py keeps two independent frames in flight on two streams (CUDA-graph replays); every library
     scratch buffer is per stream, so the concurrent results must equal the one-at-a-time results."""
     import torch
@@ -103,35 +105,16 @@ def test_two_frames_in_flight_on_two_streams(b200, refc):
 @pytest.mark.parametrize("name", ["frame_384x256", "frame_640x360", "frame_384x256_b10_m6", "frame_640x360_b10_m4"])
 def test_frame_matches_committed_golden_fixture(b200, name):
     """tests/golden/frame_WxH.json holds the SHA-256 of every output of the frame as computed by the reference's
-    own C kernels (tools/make_golden.py, run where /root/reference exists).  Needs no oracle at run time."""
-    import hashlib
+    own C kernels (tools/make_golden.py).  Needs no oracle at run time."""
     import json
     import os
-    import numpy as np
     import torch
+    import bench
     from svt_av1_psy_b200.pipeline import FramePipeline
     from svt_av1_psy_b200.workload import FrameWorkload
     g = json.load(open(os.path.join(os.path.dirname(__file__), "golden", name + ".json")))
     fp = FramePipeline(FrameWorkload(g["width"], g["height"], seed=g["seed"], bit_depth=g.get("bit_depth", 8), preset=g.get("preset", 8)), torch)
-    fp.load_inputs()
-    fp.step()
-    torch.cuda.synchronize()
-
-    def digest(t):
-        return hashlib.sha256(np.ascontiguousarray(t.cpu().numpy()).view(np.uint8).tobytes()).hexdigest()
-    got = {k: fp.me[f] for k, f in b200.ME_OUTPUT_NAMES.items()}
-    got.update({"qcoeff": fp.qcoeff, "dqcoeff": fp.dqcoeff, "eob": fp.eobs,
-           "recon": fp.recon, "cdef_mse": fp.cdef_mse, "cdef_dir": fp.cdef_dir, "cdef_out": fp.cdef_out, "wiener_M": fp.M,
-           "wiener_H": fp.Hm, "final": fp.final})
-    bad = [k for k, t in got.items() if digest(t) != g["sha256"][k]]
-    assert not bad, bad
-    # the forward coefficients only exist on the 3-call transform chain
-    s = torch.cuda.current_stream().cuda_stream
-    fp.call_residual(s)
-    fp.call_fwd_txfm(s)
-    torch.cuda.synchronize()
-    assert digest(fp.residual) == g["sha256"]["residual"]
-    assert digest(fp.coeff) == g["sha256"]["coeff"]
+    bench.check_against_golden(fp, torch)
 
 
 def test_shutdown_then_init_again_leaves_no_stale_state():

@@ -93,7 +93,7 @@ def test_install_rtcd_binds_the_reference_pointers(b200):
 @pytest.mark.parametrize("name", ["frame_384x256", "frame_384x256_b10_m6"])
 def test_reference_process_loops_with_b200_pointers_match_c_goldens(b200, name):
     """oracle/ref_driver.c's frame step = the reference's own loops around the dispatched pointers (svt_cdef_filter_fb,
-    svt_aom_inv_transform_recon*, svt_aom_copy_sb8_16, svt_av1_compute_stats*, wiener convolve ...).  Run with the B200
+    svt_aom_inv_transform_recon*, svt_aom_copy_sb8_16, svt_av1_compute_stats*, wiener convolve ...).  Run with the H100
     T1 functions installed, every output must hash to the committed C-tier fixture."""
     import ctypes as ct
     from oracle.frame_ref import RefFrame, load_workload_module
@@ -114,7 +114,7 @@ def test_reference_process_loops_with_b200_pointers_match_c_goldens(b200, name):
     outs.update({"residual": fr.residual, "coeff": fr.coeff, "qcoeff": fr.q, "dqcoeff": fr.dq,
             "eob": fr.eobs, "recon": fr.recon, "cdef_mse": fr.mse, "cdef_dir": fr.dirs, "cdef_out": fr.cdef_out, "wiener_M": fr.M, "wiener_H": fr.Hm,
             "final": fr.final})
-    # the residual kernel is not a B200 T1 pointer (it stays the reference's C function here): included because everything downstream reads it
+    # the residual kernel is not a H100 T1 pointer (it stays the reference's C function here): included because everything downstream reads it
     bad = [k for k, v in outs.items() if hashlib.sha256(np.ascontiguousarray(v).view(np.uint8).tobytes()).hexdigest() != g["sha256"][k]]
     assert not bad, bad
     enc.ref_set_tier(0)
@@ -122,7 +122,7 @@ def test_reference_process_loops_with_b200_pointers_match_c_goldens(b200, name):
 
 def test_lr_filter_unit_with_b200_pointers(b200, refc):
     """svt_av1_loop_restoration_filter_unit (restoration.c:1067) -- stripes, saved boundary lines, Wiener and self-guided --
-    with the B200 convolve / self-guided functions installed == the same call on the C tier"""
+    with the H100 convolve / self-guided functions installed == the same call on the C tier"""
     import ctypes as ct
     from test_oracle_pins import _lr_case  # the fixture generator of the a13 oracle pins
     _need_lib()
@@ -146,11 +146,11 @@ def test_lr_filter_unit_with_b200_pointers(b200, refc):
                                  dict(w=640, h=360, n=4, bd=10, preset=8, crf=30, lp=1)],
                          ids=["configs0_360p_8bit_M12", "360p_8bit_M8", "360p_10bit_M8_lp1"])
 def test_encoder_bitstream_identical_to_c_path(cfg):
-    """SURVEY.md 8(c)(ii): the encoder with the B200 tier installed writes the same bitstream as `--asm c`"""
+    """SURVEY.md 8(c)(ii): the encoder with the H100 tier installed writes the same bitstream as `--asm c`"""
     _need_lib()
     c = _encode(False, **cfg)
     g = _encode(True, **cfg)
     assert c["bytes"] > 0 and c["packets"] == cfg["n"], c
     assert g["launches"] > 10000, g  # the encode really ran on libsvtav1_b200.so
     assert (g["bytes"], g["packets"], g["sha256"]) == (c["bytes"], c["packets"], c["sha256"]), (c, g)
-    print("encode %s: C %.1fs, B200 T1 pointers %.1fs, %d kernel launches" % (cfg, c["seconds"], g["seconds"], g["launches"]))
+    print("encode %s: C %.1fs, H100 T1 pointers %.1fs, %d kernel launches" % (cfg, c["seconds"], g["seconds"], g["launches"]))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""debug helper: encode with only some kernel groups of the B200 tier installed (SVT_B200_RTCD_GROUPS) and compare with the C path"""
+"""debug helper: encode with only some kernel groups of the H100 tier installed (SVT_B200_RTCD_GROUPS) and compare with the C path"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""debug helper: one reference frame step with the B200 T1 pointers installed (REF_TRACE=1 prints the stage)"""
+"""debug helper: one reference frame step with the H100 T1 pointers installed (REF_TRACE=1 prints the stage)"""
 import ctypes as ct, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
