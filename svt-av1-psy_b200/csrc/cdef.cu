@@ -8,16 +8,20 @@
 // 106-352: CDEF_VERY_LARGE outside the frame, pre-filter neighbours inside).
 //
 // H100 mapping (T2): a frame-wide kernel finds direction and variance of every non-skip 8x8 (one
-// thread per block, the 64 pixels in registers).  Search and apply run one CTA per (64x64 filter block,
-// plane): the padded 16-bit tile of the plane is staged in shared memory once and every filtered pixel
-// is one thread.  A pixel's 12 taps are fetched once per direction, as signed differences and magnitudes
-// packed two per register, and shared by all candidate strengths; the filter sum is separable into a
-// primary and a secondary half, each evaluated once per distinct strength value with native packed
-// 16-bit min/max/add and 2-way dot-product instructions.  Distortion moments are reduced with shuffles
-// into per-block 32-bit accumulators in shared memory; the filtered pixels of the search never leave
-// registers.  The luma distortion's double-precision formula is evaluated with round-to-nearest
-// intrinsics in the reference's operand order (FMA contraction is disabled for the whole library),
-// which makes it IEEE-identical to the C code.
+// thread per block, the 64 pixels in registers).  Search and apply run one 128-thread CTA per (64x64
+// filter block, plane): the padded 16-bit tile of the plane, (fbs + 6) x (fbs + 16) for a filter block of
+// fbs x fbs pixels in that plane, is staged in shared memory once, and a thread owns a row segment of one
+// block (luma: a processed 8-pixel row of an 8x8, chroma: a 4-pixel row of a 4x4), so the tap offsets of
+// the block's direction and the per-strength constants are built once per segment, not per pixel.  A
+// pixel's 12 taps are fetched once per direction, as signed differences and magnitudes packed two per
+// register, and shared by all candidate strengths; the filter sum is separable into a primary and a
+// secondary half, each evaluated once per distinct strength value with native packed 16-bit min/max/add
+// and 2-way dot-product instructions.  The search sums a segment's distortion moments in registers (up
+// to kGChunk strengths at a time), combines the few segments of a block with shuffles and stores them once
+// per (block, strength); the source's moments and those of strength code 0 (the unfiltered block) are not
+// recomputed per strength.  The luma distortion's double-precision formula is evaluated with
+// round-to-nearest intrinsics in the reference's operand order (FMA contraction is disabled for the whole
+// library), which makes it IEEE-identical to the C code.
 #include <mutex>
 
 #include "common.cuh"
@@ -28,7 +32,6 @@ namespace b200 {
 constexpr int kVeryLarge = 0x7f7f;  // CDEF_VERY_LARGE (cdef.h:38)
 constexpr int kTP        = 88;      // tile pitch in uint16 (>= 64 + 2*8, keeps rows 16-B aligned)
 constexpr int kTileRows  = 64 + 6;
-constexpr int kGChunk    = 8;       // candidate strengths evaluated between two CTA barriers of the search
 
 __device__ __forceinline__ int msb32(uint32_t n) { return 31 - __clz(n); }
 __device__ __forceinline__ int cdef_adjust_strength(int strength, int var) {
@@ -110,74 +113,76 @@ struct CdefTaps {
     uint32_t ad[6];  // |differences|
     int      mn, mx;
 };
-__device__ __forceinline__ void cdef_load_taps(const uint16_t* in, int s, int dir, int x, CdefTaps& T) {
-    const uint32_t xx = (uint32_t)x * 0x10001u, nxx = __vneg2(xx);
-    uint32_t       mx2 = xx, mn2 = xx;
-    auto put = [&](int pair, uint32_t lo, uint32_t hi) {
-        const uint32_t p = lo | (hi << 16);
-        T.d[pair]  = __vadd2(p, nxx);
-        T.ad[pair] = __vmaxu2(p, xx) - __vminu2(p, xx);  // halves are >= 0: no borrow between them
-        // CDEF_VERY_LARGE marks "outside the picture": never the maximum.  Bit 14 tells it from a pixel.
-        const uint32_t vl = (p >> 14) & 0x00010001u;
-        mx2 = __vmaxu2(mx2, p - vl * (uint32_t)kVeryLarge);
-        mn2 = __vminu2(mn2, p);
-    };
+// element offsets of the six tap pairs along direction `dir` in a tile of pitch s (pair order as above)
+__device__ __forceinline__ void cdef_tap_offsets(int dir, int s, int (&o)[6]) {
     const int d2 = (dir + 2) & 7, d6 = (dir + 6) & 7;
 #pragma unroll
     for (int k = 0; k < 2; k++) {
-        const int po  = c_cdef_dir[dir][k][0] * s + c_cdef_dir[dir][k][1];
-        const int s0o = c_cdef_dir[d2][k][0] * s + c_cdef_dir[d2][k][1];
-        const int s2o = c_cdef_dir[d6][k][0] * s + c_cdef_dir[d6][k][1];
-        put(k, in[po], in[-po]);
-        put(2 + 2 * k, in[s0o], in[-s0o]);
-        put(3 + 2 * k, in[s2o], in[-s2o]);
+        o[k]         = c_cdef_dir[dir][k][0] * s + c_cdef_dir[dir][k][1];
+        o[2 + 2 * k] = c_cdef_dir[d2][k][0] * s + c_cdef_dir[d2][k][1];
+        o[3 + 2 * k] = c_cdef_dir[d6][k][0] * s + c_cdef_dir[d6][k][1];
+    }
+}
+__device__ __forceinline__ void cdef_load_taps(const uint16_t* in, const int (&o)[6], int x, CdefTaps& T) {
+    // CDEF_VERY_LARGE marks "outside the picture": never the maximum.  The maximum is taken over the halves
+    // plus kMxBias (mod 2^16), which maps CDEF_VERY_LARGE to 0 and keeps pixels (<= 4095) in order above it.
+    constexpr uint32_t kMxBias = 0x10000u - kVeryLarge;
+    const uint32_t xx = (uint32_t)x * 0x10001u, nxx = __vneg2(xx);
+    uint32_t       mx2 = __vadd2(xx, kMxBias * 0x10001u), mn2 = xx;
+#pragma unroll
+    for (int pair = 0; pair < 6; pair++) {
+        const uint32_t p = (uint32_t)in[o[pair]] | ((uint32_t)in[-o[pair]] << 16);
+        T.d[pair]  = __vadd2(p, nxx);
+        T.ad[pair] = __vmaxu2(p, xx) - __vminu2(p, xx);  // halves are >= 0: no borrow between them
+        mx2 = __vmaxu2(mx2, __vadd2(p, kMxBias * 0x10001u));
+        mn2 = __vminu2(mn2, p);
     }
     T.mn = (int)min(mn2 & 0xffffu, mn2 >> 16);
-    T.mx = (int)max(mx2 & 0xffffu, mx2 >> 16);
+    T.mx = (int)max(mx2 & 0xffffu, mx2 >> 16) - (int)kMxBias;
 }
-// constrain() (cdef.c:85-93) of the two taps of a pair, summed with weight w each:
-// sign(d) * min(|d|, max(0, thr - (|d| >> shift))) = clamp(d, -m, m) with m = thr - min(|d| >> shift, thr).
-// A zero threshold gives m = 0 and so zero by itself.  The reference accumulates in int16; |sum| <=
-// 2*(4+2)*240 + 4*(2+1)*64 for 12-bit content, so the int32 sum is the same number.
-__device__ __forceinline__ int cdef_pair_sum(const CdefTaps& T, int pair, uint32_t thr2, int sh, uint32_t shmask, int wbytes, int acc) {
-    const uint32_t t1 = (T.ad[pair] >> sh) & shmask;
-    const uint32_t m  = thr2 - __vminu2(t1, thr2);
-    const uint32_t v  = __vmins2(__vmaxs2(T.d[pair], __vneg2(m)), m);
-    return __dp2a_lo((int)v, wbytes, acc);
+// What constrain() (cdef.c:85-93) needs of a strength t at a damping: the threshold in both halves, the shift
+// max(0, damping - msb(t)), the mask that keeps the shifted high half out of the low one, and the dp2a
+// weights of the two primary pairs (byte pair 0-1: k = 0, 2-3: k = 1; cdef_pri_taps[(t >> coeff_shift) & 1]).
+// t = 0 gives a zero threshold, which constrains every tap to zero.
+__device__ __forceinline__ uint4 cdef_strength_consts(int t, int damping, int coeff_shift) {
+    const int sh = max(0, damping - msb32((uint32_t)t));
+    return make_uint4((uint32_t)t * 0x10001u, (uint32_t)sh, (0xffffu >> sh) * 0x10001u,
+                      ((t >> coeff_shift) & 1) ? 0x03030303u : 0x02020404u);
+}
+// constrain() of the two taps of a pair: sign(d) * min(|d|, max(0, thr - (|d| >> shift))) = clamp(d, -m, m)
+// with m = thr - min(|d| >> shift, thr), as two signed 16-bit halves.
+__device__ __forceinline__ uint32_t cdef_constrain2(const CdefTaps& T, int pair, const uint4& c) {
+    const uint32_t t1 = (T.ad[pair] >> c.y) & c.z;
+    const uint32_t m  = c.x - __vminu2(t1, c.x);
+    return __vmins2(__vmaxs2(T.d[pair], __vneg2(m)), m);
 }
 // The sum splits into a primary part (4 taps, depends on the primary strength only) and a secondary part
 // (8 taps, depends on the secondary strength only): candidate strengths that share one of the two share
-// that half of the work.
-__device__ __forceinline__ int cdef_primary_sum(const CdefTaps& T, int pri, int pri_damping, int coeff_shift) {
-    const int      sh = max(0, pri_damping - msb32((uint32_t)pri));
-    const uint32_t thr2 = (uint32_t)pri * 0x10001u, shmask = (0xffffu >> sh) * 0x10001u;
-    const int      odd = (pri >> coeff_shift) & 1;
-    int            sum = cdef_pair_sum(T, 0, thr2, sh, shmask, odd ? 0x0303 : 0x0404, 0);
-    return cdef_pair_sum(T, 1, thr2, sh, shmask, odd ? 0x0303 : 0x0202, sum);
+// that half of the work.  The reference accumulates in int16; |sum| <= 2*(4+2)*240 + 4*(2+1)*64 for 12-bit
+// content, so the int32 sum is the same number.  Two constrained secondary taps (|v| <= 64 each) add
+// without overflow in a 16-bit half.
+__device__ __forceinline__ int cdef_primary_sum(const CdefTaps& T, const uint4& c) {
+    return __dp2a_hi((int)cdef_constrain2(T, 1, c), (int)c.w, __dp2a_lo((int)cdef_constrain2(T, 0, c), (int)c.w, 0));
 }
-__device__ __forceinline__ int cdef_secondary_sum(const CdefTaps& T, int sec, int sec_damping) {
-    const int      sh = max(0, sec_damping - msb32((uint32_t)sec));
-    const uint32_t thr2 = (uint32_t)sec * 0x10001u, shmask = (0xffffu >> sh) * 0x10001u;
-    int            sum = cdef_pair_sum(T, 2, thr2, sh, shmask, 0x0202, 0);
-    sum = cdef_pair_sum(T, 3, thr2, sh, shmask, 0x0202, sum);
-    sum = cdef_pair_sum(T, 4, thr2, sh, shmask, 0x0101, sum);
-    return cdef_pair_sum(T, 5, thr2, sh, shmask, 0x0101, sum);
+__device__ __forceinline__ int cdef_secondary_sum(const CdefTaps& T, const uint4& c) {
+    const uint32_t w2 = __vadd2(cdef_constrain2(T, 2, c), cdef_constrain2(T, 3, c));
+    const uint32_t w1 = __vadd2(cdef_constrain2(T, 4, c), cdef_constrain2(T, 5, c));
+    return __dp2a_lo((int)w2, 0x0202, __dp2a_lo((int)w1, 0x0101, 0));
 }
 __device__ __forceinline__ int cdef_finish_px(const CdefTaps& T, int x, int sum) {
     const int y = x + ((8 + sum - (sum < 0)) >> 4);
     return y < T.mn ? T.mn : (y > T.mx ? T.mx : y);
 }
-__device__ __forceinline__ int cdef_eval_taps(const CdefTaps& T, int x, int pri, int sec, int pri_damping, int sec_damping,
-                                              int coeff_shift) {
-    return cdef_finish_px(T, x, cdef_primary_sum(T, pri, pri_damping, coeff_shift) + cdef_secondary_sum(T, sec, sec_damping));
-}
 // one filtered pixel; `in` points at the pixel, s = tile pitch
 __device__ __forceinline__ int cdef_filter_px(const uint16_t* in, int s, int pri_strength, int sec_strength, int dir,
                                               int pri_damping, int sec_damping, int coeff_shift) {
     CdefTaps  T;
+    int       o[6];
     const int x = in[0];
-    cdef_load_taps(in, s, dir, x, T);
-    return cdef_eval_taps(T, x, pri_strength, sec_strength, pri_damping, sec_damping, coeff_shift);
+    cdef_tap_offsets(dir, s, o);
+    cdef_load_taps(in, o, x, T);
+    return cdef_finish_px(T, x, cdef_primary_sum(T, cdef_strength_consts(pri_strength, pri_damping, coeff_shift)) +
+                                    cdef_secondary_sum(T, cdef_strength_consts(sec_strength, sec_damping, coeff_shift)));
 }
 
 // luma psy distortion of one 8xN block from its five moments (enc_cdef.c:41-47); exact IEEE sequence
@@ -290,28 +295,57 @@ __global__ void search_one_dual_kernel(const unsigned long long* mse0, const uns
 // ------------------------------------------------------------------------------------------------
 // T2: per-filter-block search (all planes, all candidate strengths) and frame apply
 // ------------------------------------------------------------------------------------------------
+constexpr int kT2Threads = 128;  // threads of a search / apply CTA
+constexpr int kGChunk    = 8;    // candidate strengths whose moments a search thread keeps in registers at once
+
 template <typename PIX>
-__device__ void stage_cdef_tile(uint16_t* tile, const PIX* plane, int stride, int plane_w, int plane_h, int fbr, int fbc,
-                                int nvfb, int nhfb, int bw, int bh, int vsz, int hsz) {
+__device__ void stage_cdef_tile(uint16_t* tile, const PIX* plane, int stride, int fbr, int fbc, int nvfb, int nhfb, int fbs,
+                                int vsz, int hsz) {
     // tile origin (row 3, col 8) = first pixel of the filter block; everything outside the copied
-    // rectangle is CDEF_VERY_LARGE (cdef_process.c:211-230).  One pass, two pixels per thread and store.
+    // rectangle is CDEF_VERY_LARGE (cdef_process.c:211-230).  Only the (fbs + 6) x (fbs + 16) pixels the
+    // filter can read are written.  One pass, two pixels per thread and store.
     const int yoff = 3 * (fbr != 0), xoff = 8 * (fbc != 0);
     const int ysize = vsz + 3 * (fbr + 1 < nvfb) + yoff, xsize = hsz + 8 * (fbc + 1 < nhfb) + xoff;
-    (void)plane_w; (void)plane_h;
-    const int py0 = fbr * bh - yoff, px0 = fbc * bw - xoff;
-    constexpr int kPairs = (64 + 16) / 2;  // columns 0..79 are the ones ever read
+    const int py0 = fbr * fbs - yoff, px0 = fbc * fbs - xoff;
+    const int pairs = (fbs + 16) / 2;
+    // a pair starts at an even column: one load per pair when the plane's rows are aligned to it
+    const bool pair_load = (((size_t)plane | (size_t)stride * sizeof(PIX)) & (2 * sizeof(PIX) - 1)) == 0;
 #pragma unroll 4
-    for (int i = threadIdx.x; i < kTileRows * kPairs; i += blockDim.x) {
-        const int r = i / kPairs, c = (i - r * kPairs) * 2;
+    for (int i = threadIdx.x; i < (fbs + 6) * pairs; i += blockDim.x) {
+        const int r = i / pairs, c = (i - r * pairs) * 2;
         const int rr = r - (3 - yoff), cc = c - (8 - xoff);  // cc is even, xsize is a multiple of 4: the pair is in or out together
         uint32_t v = (uint32_t)kVeryLarge * 0x10001u;
         if (rr >= 0 && rr < ysize && cc >= 0 && cc < xsize) {
             const PIX* p = plane + (size_t)(py0 + rr) * stride + px0 + cc;
-            v = (uint32_t)p[0] | ((uint32_t)p[1] << 16);
+            if (!pair_load) v = (uint32_t)p[0] | ((uint32_t)p[1] << 16);
+            else if (sizeof(PIX) == 1) v = __byte_perm(*reinterpret_cast<const uint16_t*>(p), 0, 0x4140);  // 0, p[1], 0, p[0]
+            else v = *reinterpret_cast<const uint32_t*>(p);
         }
         *reinterpret_cast<uint32_t*>(tile + r * kTP + c) = v;
     }
     __syncthreads();
+}
+
+// Ordered list of the non-skip 8x8s of filter block (fbr, fbc) (svt_sb_compute_cdef_list: by*8+bx, raster
+// order) and their directions / variances, into shared memory.  Threads 0..63 (two whole warps) take part;
+// the caller synchronises before the list is read.  Returns the count (read from the ballots: CTA-uniform).
+__device__ __forceinline__ int cdef_fb_list(const uint8_t* skip8x8, const uint8_t* dir_in, const int* var_in, int fb, int fbr,
+                                            int fbc, int w8, int h8, uint8_t* s_list, uint8_t* s_dir, int* s_var, unsigned* s_ballot) {
+    if (threadIdx.x < 64) {
+        const int  by = threadIdx.x >> 3, bx = threadIdx.x & 7, gy = fbr * 8 + by, gx = fbc * 8 + bx;
+        const bool on = gy < h8 && gx < w8 && !skip8x8[gy * w8 + gx];
+        const unsigned m = __ballot_sync(0xffffffffu, on);
+        s_dir[threadIdx.x] = dir_in[(size_t)fb * 64 + threadIdx.x];
+        s_var[threadIdx.x] = var_in[(size_t)fb * 64 + threadIdx.x];
+        if ((threadIdx.x & 31) == 0) s_ballot[threadIdx.x >> 5] = m;
+    }
+    __syncthreads();
+    const unsigned m0 = s_ballot[0], m1 = s_ballot[1];
+    if (threadIdx.x < 64) {
+        const unsigned mine = threadIdx.x < 32 ? m0 : m1, lane = threadIdx.x & 31;
+        if ((mine >> lane) & 1) s_list[(threadIdx.x < 32 ? 0 : __popc(m0)) + __popc(mine & ((1u << lane) - 1))] = (uint8_t)threadIdx.x;
+    }
+    return __popc(m0) + __popc(m1);
 }
 
 // direction + variance of every non-skip 8x8 luma block of the frame: one thread per block
@@ -332,48 +366,203 @@ cdef_dir_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, uint8_t
     var_out[o] = var;
 }
 
+// One chunk of candidate strengths (CTA-uniform description) as the search's threads see it.
+struct CdefChunk {
+    int      sv[kGChunk];  // strength codes, -1 = not tested (also past the end of the list)
+    unsigned todo[2];      // pass 0: taps along the block's direction (a primary part, or code 0); pass 1: along direction 0
+    unsigned pri_new;      // pass-0 strengths whose primary code differs from the previous one with a primary part
+    unsigned secs[2];      // per pass: bit c set when secondary code c (1..3) occurs
+};
+
+// Moments of one row segment (BS pixels at `in`, source at `o_row`) for every strength of `todo`, the
+// taps along one direction.  Luma (BS = 8) accumulates sum y, y^2, y*src; chroma (BS = 4) sum (src - y)^2.
+// Taps are loaded once per pixel and shared by all strengths; the primary half is recomputed only when the
+// primary strength changes and the secondary half once per distinct secondary code.
+template <int BS, typename PIX>
+__device__ __forceinline__ void cdef_segment_pass(const uint16_t* in, const PIX* o_row, const int (&off)[6], const CdefChunk& C, int pass,
+                                                  const int (&tadj)[kGChunk], const uint4* tab, int cs, unsigned (&a0)[kGChunk],
+                                                  unsigned (&a1)[kGChunk], unsigned (&a2)[kGChunk]) {
+    const unsigned todo = C.todo[pass], pnew = pass ? 0u : C.pri_new, secs = C.secs[pass];
+#pragma unroll 1
+    for (int j = 0; j < BS; j++) {
+        const int      x = in[j];
+        const unsigned o = o_row[j];
+        CdefTaps       T;
+        cdef_load_taps(in + j, off, x, T);
+        int s1 = 0, s2 = 0, s3 = 0;  // secondary halves of codes 1, 2, 3 (strengths 1, 2, 4 << cs)
+        if (secs & 2) s1 = cdef_secondary_sum(T, tab[1 << cs]);
+        if (secs & 4) s2 = cdef_secondary_sum(T, tab[2 << cs]);
+        if (secs & 8) s3 = cdef_secondary_sum(T, tab[4 << cs]);
+        int psum = 0;
+#pragma unroll
+        for (int gi = 0; gi < kGChunk; gi++) {
+            if (!((todo >> gi) & 1)) continue;  // CTA-uniform
+            if ((pnew >> gi) & 1) psum = cdef_primary_sum(T, tab[tadj[gi]]);
+            const int sc = C.sv[gi] & 3, ssum = sc == 1 ? s1 : (sc == 2 ? s2 : (sc == 3 ? s3 : 0));
+            // code 0 leaves the pixel unchanged (sum = 0, and x lies inside [min, max] of its own neighbourhood)
+            const unsigned y = C.sv[gi] == 0 ? (unsigned)x : (unsigned)cdef_finish_px(T, x, psum + ssum);
+            if (BS == 8) {
+                a0[gi] += y;
+                a1[gi] += y * y;
+                a2[gi] += y * o;
+            } else {
+                const int e = (int)o - (int)y;
+                a0[gi] += (unsigned)(e * e);
+            }
+        }
+    }
+}
+
+// The strength search of one (filter block, plane): every thread owns processed row segments (luma: one
+// 8-pixel row of an 8x8, chroma: one 4-pixel row of a 4x4), so tap offsets and strength constants are
+// built once per segment, and only the R threads of a block combine their moments, by shuffles.  Their
+// sums go to shared memory once per (block, strength); warps then turn them into distortions (luma: the
+// psy formula on the five moments) and sum them over the blocks.
+template <int BS, typename PIX>
+__device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4* tab, const PIX* src, int sstride, const int* strengths,
+                                               int n_strengths, int count, int subs, int cs, int pli, const uint8_t* s_list,
+                                               const uint8_t* s_dir, const int* s_var, unsigned (*s_mom)[3][64], unsigned (*s_src)[64],
+                                               unsigned long long* mse_fb) {
+    const int R = BS / subs, nseg = count * R;  // processed rows per block (a power of two: R divides 32)
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int g0 = 0; g0 < n_strengths; g0 += kGChunk) {
+        const int ng = min(kGChunk, n_strengths - g0);
+        CdefChunk C;
+        C.todo[0] = C.todo[1] = C.pri_new = C.secs[0] = C.secs[1] = 0;
+        unsigned zero = 0;
+        int      last_pri = -1;
+#pragma unroll
+        for (int gi = 0; gi < kGChunk; gi++) {
+            const int sv = gi < ng ? strengths[g0 + gi] : -1;
+            C.sv[gi] = sv;
+            if (sv < 0) continue;
+            const int pri = sv >> 2, sc = sv & 3;
+            if (pri) {
+                C.todo[0] |= 1u << gi;
+                C.secs[0] |= (1u << sc) & ~1u;
+                if (pri != last_pri) C.pri_new |= 1u << gi;
+                last_pri = pri;
+            } else if (sc) {
+                C.todo[1] |= 1u << gi;
+                C.secs[1] |= 1u << sc;
+            } else {
+                zero |= 1u << gi;
+            }
+        }
+        // code 0 needs no taps: it joins a pass that runs anyway
+        if (C.todo[0] || !C.todo[1]) C.todo[0] |= zero;
+        else C.todo[1] |= zero;
+        const unsigned tested = C.todo[0] | C.todo[1];
+        for (int s = threadIdx.x; s < ((nseg + 31) & ~31); s += kT2Threads) {  // whole warps stay in the loop (shuffles)
+            const bool live = s < nseg;
+            const int  bi = live ? s / R : 0, r = live ? s - bi * R : 0;
+            const int  b = s_list[bi], by = b >> 3, bx = b & 7, row = BS * by + r * subs;
+            const uint16_t* in    = tile + (3 + row) * kTP + 8 + BS * bx;
+            const PIX*      o_row = src + (size_t)row * sstride + BS * bx;
+            unsigned a0[kGChunk], a1[kGChunk], a2[kGChunk];
+#pragma unroll
+            for (int gi = 0; gi < kGChunk; gi++) a0[gi] = a1[gi] = a2[gi] = 0;
+            int tadj[kGChunk];  // the adjusted primary strength of each pass-0 strength that starts a new primary half
+            const int var = s_var[b];
+#pragma unroll
+            for (int gi = 0; gi < kGChunk; gi++) {
+                const int pri = (C.sv[gi] >> 2) << cs;
+                tadj[gi] = (C.pri_new >> gi) & 1 ? (BS == 4 ? pri : cdef_adjust_strength(pri, var)) : 0;
+            }
+            int off[6];
+            if (C.todo[0]) {
+                cdef_tap_offsets(s_dir[b], kTP, off);
+                cdef_segment_pass<BS, PIX>(in, o_row, off, C, 0, tadj, tab, cs, a0, a1, a2);
+            }
+            if (C.todo[1]) {
+                cdef_tap_offsets(0, kTP, off);
+                cdef_segment_pass<BS, PIX>(in, o_row, off, C, 1, tadj, tab, cs, a0, a1, a2);
+            }
+            const bool lead = live && r == 0;
+#pragma unroll
+            for (int gi = 0; gi < kGChunk; gi++) {
+                if (!((tested >> gi) & 1)) continue;  // CTA-uniform
+                for (int sh = R >> 1; sh > 0; sh >>= 1) {
+                    a0[gi] += __shfl_xor_sync(0xffffffffu, a0[gi], sh);
+                    if (BS == 8) {
+                        a1[gi] += __shfl_xor_sync(0xffffffffu, a1[gi], sh);
+                        a2[gi] += __shfl_xor_sync(0xffffffffu, a2[gi], sh);
+                    }
+                }
+                if (lead) {
+                    s_mom[gi][0][bi] = a0[gi];
+                    if (BS == 8) {
+                        s_mom[gi][1][bi] = a1[gi];
+                        s_mom[gi][2][bi] = a2[gi];
+                    }
+                }
+            }
+            if (BS == 8 && g0 == 0) {  // the source's moments do not depend on the strength
+                unsigned so = 0, so2 = 0;
+#pragma unroll
+                for (int j = 0; j < BS; j++) {
+                    const unsigned o = o_row[j];
+                    so += o;
+                    so2 += o * o;
+                }
+                for (int sh = R >> 1; sh > 0; sh >>= 1) {
+                    so += __shfl_xor_sync(0xffffffffu, so, sh);
+                    so2 += __shfl_xor_sync(0xffffffffu, so2, sh);
+                }
+                if (lead) {
+                    s_src[0][bi] = so;
+                    s_src[1][bi] = so2;
+                }
+            }
+        }
+        __syncthreads();
+        // per strength: the blocks' distortions, summed by one warp
+        for (int gi = warp; gi < ng; gi += kT2Threads / 32) {
+            const int          sv = strengths[g0 + gi];
+            unsigned long long acc = 0;
+            if (sv >= 0)
+                for (int bi = lane; bi < count; bi += 32)
+                    acc += BS == 8 ? cdef_dist_from_sums(s_mom[gi][0][bi], s_src[0][bi], s_mom[gi][1][bi], s_src[1][bi], s_mom[gi][2][bi], cs)
+                                   : (unsigned long long)s_mom[gi][0][bi];
+#pragma unroll
+            for (int sh = 16; sh > 0; sh >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, sh);
+            if (lane == 0) {
+                unsigned long long* m = mse_fb + g0 + gi;
+                // enc: mse_seg = (sum >> 2*coeff_shift) * subsampling_factor; untested chroma = default_mse_uv*64
+                const unsigned long long v = sv >= 0 ? (acc >> (2 * cs)) * (unsigned long long)subs : 0;
+                if (pli == 0) *m = v;
+                else atomicAdd(m, sv < 0 ? (pli == 1 ? 1040400ull * 64ull : 0ull) : v);
+            }
+        }
+        __syncthreads();  // s_mom is reused by the next chunk
+    }
+}
+
 // Strength search: one CTA per (filter block, plane).  mse[1] (chroma) must be zero on entry: the two
 // chroma planes add into it.
 template <typename PIX>
-__global__ void __launch_bounds__(256, 3)
+__global__ void __launch_bounds__(kT2Threads, 5)
 cdef_search_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const int* __restrict__ strengths_y,
                    const int* __restrict__ strengths_uv, int n_strengths, unsigned long long* __restrict__ mse /*[2][nfb][n_strengths]*/,
                    const uint8_t* __restrict__ dir_in /*[nfb][64]*/, const int* __restrict__ var_in /*[nfb][64]*/) {
-    __shared__ uint16_t tile[kTileRows * kTP];
+    __shared__ __align__(16) uint16_t tile[kTileRows * kTP];
+    __shared__ uint4    s_tab[2][256];  // cdef_strength_consts of every strength value, luma / chroma damping
     __shared__ uint8_t  s_dir[64];
     __shared__ int      s_var[64];
-    __shared__ uint8_t  s_list[64];  // by*8+bx of the non-skip 8x8s, raster order (svt_sb_compute_cdef_list)
-    __shared__ int      s_count;
+    __shared__ uint8_t  s_list[64];
     __shared__ unsigned s_ballot[2];
-    __shared__ int                s_sv[kGChunk];          // the chunk's strength codes (-1 = not tested)
-    __shared__ unsigned long long s_dist[kGChunk][64];    // per strength, per block: distortion
-    __shared__ unsigned int       s_blk[kGChunk][64][5];  // per strength, per block: luma sum_s, sum_d, sum_s2, sum_d2, sum_sd; chroma [0] = sse
+    __shared__ unsigned s_mom[kGChunk][3][64];  // per strength, per listed block: luma sum y, y^2, y*src; chroma [0] = sum (src - y)^2
+    __shared__ unsigned s_src[2][64];           // per listed luma block: sum src, src^2
     const int nhfb = (f.width + 63) >> 6, nvfb = (f.height + 63) >> 6, nfb = nhfb * nvfb;
     const int cs = f.bit_depth > 8 ? f.bit_depth - 8 : 0;
     const int w8 = (f.width + 7) >> 3, h8 = (f.height + 7) >> 3;
+    // strengths reach (15 << 4) = 240 (primary, 12-bit), adjusted ones no more, secondary 4 << 4
+    for (int i = threadIdx.x; i < 2 * 256; i += kT2Threads) s_tab[i >> 8][i & 255] = cdef_strength_consts(i & 255, f.damping + cs - (i >> 8), cs);
     for (int work = blockIdx.x; work < nfb * 3; work += gridDim.x) {
         const int fb = work / 3, pli = work - fb * 3;
         const int fbr = fb / nhfb, fbc = fb - fbr * nhfb;
         __syncthreads();
-        if (threadIdx.x < 64) {  // ordered list of the non-skip blocks: ballot + prefix count
-            const int  by = threadIdx.x >> 3, bx = threadIdx.x & 7, gy = fbr * 8 + by, gx = fbc * 8 + bx;
-            const bool on = gy < h8 && gx < w8 && !skip8x8[gy * w8 + gx];
-            const unsigned m = __ballot_sync(0xffffffffu, on);
-            s_dir[threadIdx.x] = dir_in[(size_t)fb * 64 + threadIdx.x];
-            s_var[threadIdx.x] = var_in[(size_t)fb * 64 + threadIdx.x];
-            if ((threadIdx.x & 31) == 0) s_ballot[threadIdx.x >> 5] = m;
-        }
-        __syncthreads();
-        {
-            const unsigned m0 = s_ballot[0], m1 = s_ballot[1];
-            if (threadIdx.x < 64) {
-                const unsigned mine = threadIdx.x < 32 ? m0 : m1, lane = threadIdx.x & 31;
-                if ((mine >> lane) & 1) s_list[(threadIdx.x < 32 ? 0 : __popc(m0)) + __popc(mine & ((1u << lane) - 1))] = (uint8_t)threadIdx.x;
-            }
-            if (threadIdx.x == 0) s_count = __popc(m0) + __popc(m1);
-        }
-        __syncthreads();
-        const int count = s_count;
+        const int count = cdef_fb_list(skip8x8, dir_in, var_in, fb, fbr, fbc, w8, h8, s_list, s_dir, s_var, s_ballot);
         if (count == 0) {
             if (pli == 0)
                 for (int g = threadIdx.x; g < n_strengths; g += blockDim.x) mse[(size_t)fb * n_strengths + g] = 0;
@@ -385,133 +574,73 @@ cdef_search_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, cons
         const int rstride = pli ? f.recon_stride_c : f.recon_stride_y, sstride = pli ? f.src_stride_c : f.src_stride_y;
         const int pw = f.width >> dec, ph = f.height >> dec, fbs = 64 >> dec;
         const int hsz = min(fbs, pw - fbc * fbs), vsz = min(fbs, ph - fbr * fbs);
-        stage_cdef_tile<PIX>(tile, rec, rstride, pw, ph, fbr, fbc, nvfb, nhfb, fbs, fbs, vsz, hsz);
-        const int bsz = 8 >> dec;                       // block edge in this plane
-        int subs = f.subsampling_factor;
-        subs = min(subs, dec ? 1 : 4);                  // cdef_process.c:243-248 (4:2:0 chroma = BLOCK_4X4)
-        const int rows_per_blk = bsz / subs;
-        const int damping = f.damping + cs - (pli != 0);
-        const int* strengths = pli ? strengths_uv : strengths_y;
-        // One thread per filtered pixel: idx -> (block, processed row, column), so a warp reads whole
-        // 8- (4-) pixel row segments of the tile and of the source picture.  The taps of a pixel are
-        // fetched once per direction (the block's own for strengths with a primary part, direction 0
-        // for the others) and shared by all candidate strengths; strengths are taken kGChunk at a
-        // time, each with its own accumulators, so the CTA synchronises per chunk, not per strength.
-        const int ppb = bsz * rows_per_blk, lg_bsz = 3 - dec;  // processed pixels per block: 64/32/16 (luma), 16 (chroma)
-        const int seg = min(ppb, 32);                          // lanes that share a block
-        for (int g0 = 0; g0 < n_strengths; g0 += kGChunk) {
-            const int ng = min(kGChunk, n_strengths - g0);
-            for (int i = threadIdx.x; i < kGChunk * 64 * 5; i += blockDim.x) (&s_blk[0][0][0])[i] = 0;
-            if ((int)threadIdx.x < ng) s_sv[threadIdx.x] = strengths[g0 + threadIdx.x];
-            unsigned with_pri = 0, without_pri = 0;  // which strengths of the chunk have / lack a primary part
-            bool     sec_without_pri = false;         // ... and whether any of the latter has a secondary part
-            for (int gi = 0; gi < ng; gi++) {
-                const int sv = strengths[g0 + gi];
-                if (sv >= 0) (sv / 4 ? with_pri : without_pri) |= 1u << gi;
-                if (sv > 0 && sv / 4 == 0) sec_without_pri = true;
-            }
-            __syncthreads();
-            for (int idx = threadIdx.x; idx < ((count * ppb + 31) & ~31); idx += blockDim.x) {  // whole warps stay in the loop (shuffles)
-                const bool live = idx < count * ppb;
-                const int  bi = live ? idx / ppb : 0, within = idx - (idx / ppb) * ppb;
-                const int  ri = (within >> lg_bsz) * subs, j = within & (bsz - 1);
-                const int  b = s_list[bi], by = b >> 3, bx = b & 7;
-                const uint16_t* in = tile + (3 + bsz * by + ri) * kTP + 8 + bsz * bx + j;
-                const unsigned int o = live ? (unsigned int)src[(size_t)(fbr * fbs + bsz * by + ri) * sstride + fbc * fbs + bsz * bx + j] : 0u;
-                const int x = in[0], var = s_var[b], dirb = s_dir[b];
-#pragma unroll 1
-                for (int pass = 0; pass < 2; pass++) {
-                    const unsigned todo = pass ? without_pri : with_pri;
-                    if (!todo) continue;  // CTA-uniform
-                    // a candidate with neither a primary nor a secondary part leaves the pixel unchanged
-                    // (sum = 0, and x lies inside [min, max] of its own neighbourhood): no taps needed
-                    CdefTaps T;
-                    const bool taps = pass == 0 || sec_without_pri;  // CTA-uniform
-                    if (taps) cdef_load_taps(in, kTP, pass ? 0 : dirb, x, T);
-                    // the primary half is recomputed when the primary strength changes, the secondary half
-                    // once per distinct secondary code (0..3) of this pass
-                    int last_pri = -1, psum = 0, sec1 = 0, sec2 = 0, sec3 = 0;
-                    unsigned have = 0;
-#pragma unroll 1
-                    for (int gi = 0; gi < ng; gi++) {
-                        if (!((todo >> gi) & 1)) continue;  // CTA-uniform
-                        const int sv = s_sv[gi];
-                        const int pri_code = sv >> 2, sec_code = sv & 3;  // sv >= 0 here
-                        if (pri_code != last_pri) {  // CTA-uniform
-                            const int pri = pri_code << cs;
-                            psum     = pri_code ? cdef_primary_sum(T, pli ? pri : cdef_adjust_strength(pri, var), damping, cs) : 0;
-                            last_pri = pri_code;
-                        }
-                        int ssum = 0;
-                        if (sec_code) {  // CTA-uniform
-                            if (!((have >> sec_code) & 1)) {
-                                const int v = cdef_secondary_sum(T, (sec_code + (sec_code == 3)) << cs, damping);
-                                if (sec_code == 1) sec1 = v;
-                                else if (sec_code == 2) sec2 = v;
-                                else sec3 = v;
-                                have |= 1u << sec_code;
-                            }
-                            ssum = sec_code == 1 ? sec1 : (sec_code == 2 ? sec2 : sec3);
-                        }
-                        const unsigned int y = live ? (unsigned int)(taps ? cdef_finish_px(T, x, psum + ssum) : x) : 0u;
-                        if (pli == 0) {
-                            // five moments of the block (<= 64 pixels of <= 12 bits: fit 32 bits)
-                            unsigned int ss = y, sdv = o, s2 = y * y, d2 = o * o, sdp = y * o;
-                            for (int sh = seg >> 1; sh > 0; sh >>= 1) {
-                                ss += __shfl_xor_sync(0xffffffffu, ss, sh);
-                                sdv += __shfl_xor_sync(0xffffffffu, sdv, sh);
-                                s2 += __shfl_xor_sync(0xffffffffu, s2, sh);
-                                d2 += __shfl_xor_sync(0xffffffffu, d2, sh);
-                                sdp += __shfl_xor_sync(0xffffffffu, sdp, sh);
-                            }
-                            if (live && (idx & (seg - 1)) == 0) {
-                                unsigned int* sb = s_blk[gi][bi];
-                                atomicAdd(sb + 0, ss);
-                                atomicAdd(sb + 1, sdv);
-                                atomicAdd(sb + 2, s2);
-                                atomicAdd(sb + 3, d2);
-                                atomicAdd(sb + 4, sdp);
-                            }
-                        } else {
-                            const int e = (int)o - (int)y;
-                            unsigned int se = (unsigned int)(e * e);  // a block's 16 pixels of <= 12 bits: fits 32 bits
-                            for (int sh = seg >> 1; sh > 0; sh >>= 1) se += __shfl_xor_sync(0xffffffffu, se, sh);
-                            if (live && (idx & (seg - 1)) == 0 && se) atomicAdd(&s_blk[gi][bi][0], se);
-                        }
-                    }
-                }
-            }
-            __syncthreads();
-            // per (strength, block): the block's distortion (luma: the psy formula on its five moments)
-            for (int q = threadIdx.x; q < ng * count; q += blockDim.x) {
-                const int gi = q / count, bi = q - gi * count;
-                const unsigned int* sb = s_blk[gi][bi];
-                s_dist[gi][bi] = pli == 0 ? cdef_dist_from_sums(sb[0], sb[1], sb[2], sb[3], sb[4], cs) : (unsigned long long)sb[0];
-            }
-            __syncthreads();
-            if ((int)threadIdx.x < ng) {
-                const int g = g0 + threadIdx.x, sv = s_sv[threadIdx.x];
-                unsigned long long acc = 0;
-                for (int bi = 0; bi < count; bi++) acc += s_dist[threadIdx.x][bi];
-                unsigned long long* m = mse + (size_t)((pli ? 1 : 0) * nfb + fb) * n_strengths + g;
-                // enc: mse_seg = (sum >> 2*coeff_shift) * subsampling_factor; untested chroma = default_mse_uv*64
-                const unsigned long long v = sv >= 0 ? (acc >> (2 * cs)) * (unsigned long long)subs : 0;
-                if (pli == 0) *m = v;
-                else atomicAdd(m, sv < 0 ? (pli == 1 ? 1040400ull * 64ull : 0ull) : v);
-            }
-            __syncthreads();
+        stage_cdef_tile<PIX>(tile, rec, rstride, fbr, fbc, nvfb, nhfb, fbs, vsz, hsz);  // ends with a barrier
+        const PIX* src_fb = src + (size_t)fbr * fbs * sstride + fbc * fbs;
+        unsigned long long* mse_fb = mse + (size_t)((pli ? 1 : 0) * nfb + fb) * n_strengths;
+        const int subs = min(f.subsampling_factor, dec ? 1 : 4);  // cdef_process.c:243-248 (4:2:0 chroma = BLOCK_4X4)
+        if (pli == 0)
+            cdef_search_fb<8, PIX>(tile, s_tab[0], src_fb, sstride, strengths_y, n_strengths, count, subs, cs, pli, s_list, s_dir, s_var,
+                                   s_mom, s_src, mse_fb);
+        else
+            cdef_search_fb<4, PIX>(tile, s_tab[1], src_fb, sstride, strengths_uv, n_strengths, count, subs, cs, pli, s_list, s_dir, s_var,
+                                   s_mom, s_src, mse_fb);
+    }
+}
+
+// BS filtered pixels to one row of a picture, with one store when the row is aligned to it
+template <int BS, typename PIX>
+__device__ __forceinline__ void cdef_store_row(PIX* p, const int (&y)[BS], bool wide) {
+    constexpr int NW = BS * (int)sizeof(PIX) / 4;  // 32-bit words in the row
+    if (wide) {
+        uint32_t w[NW];
+#pragma unroll
+        for (int k = 0; k < NW; k++) {
+            if (sizeof(PIX) == 1)
+                w[k] = (uint32_t)y[4 * k] | ((uint32_t)y[4 * k + 1] << 8) | ((uint32_t)y[4 * k + 2] << 16) | ((uint32_t)y[4 * k + 3] << 24);
+            else
+                w[k] = (uint32_t)y[2 * k] | ((uint32_t)y[2 * k + 1] << 16);
         }
+        if (NW == 1) *reinterpret_cast<uint32_t*>(p) = w[0];
+        else if (NW == 2) *reinterpret_cast<uint2*>(p) = make_uint2(w[0], w[1 % NW]);
+        else *reinterpret_cast<uint4*>(p) = make_uint4(w[0], w[1 % NW], w[2 % NW], w[3 % NW]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < BS; j++) p[j] = (PIX)y[j];
+    }
+}
+
+// the filter of one (filter block, plane) with one strength: a thread per BS-pixel row of a block
+template <int BS, typename PIX>
+__device__ __forceinline__ void cdef_apply_fb(const uint16_t* tile, PIX* out_fb, int ostride, bool wide, int count, int pri, int sec,
+                                              int damping, int cs, const uint8_t* s_list, const uint8_t* s_dir, const int* s_var) {
+    const uint4 csec = cdef_strength_consts(sec, damping, cs);
+    for (int s = threadIdx.x; s < count * BS; s += kT2Threads) {
+        const int bi = s / BS, r = s - bi * BS;
+        const int b = s_list[bi], by = b >> 3, bx = b & 7;
+        const uint4 cpri = cdef_strength_consts(BS == 4 ? pri : cdef_adjust_strength(pri, s_var[b]), damping, cs);
+        int off[6];
+        cdef_tap_offsets(pri ? s_dir[b] : 0, kTP, off);
+        const uint16_t* in = tile + (3 + BS * by + r) * kTP + 8 + BS * bx;
+        int y[BS];
+#pragma unroll
+        for (int j = 0; j < BS; j++) {
+            CdefTaps  T;
+            const int x = in[j];
+            cdef_load_taps(in + j, off, x, T);
+            y[j] = cdef_finish_px(T, x, (pri ? cdef_primary_sum(T, cpri) : 0) + (sec ? cdef_secondary_sum(T, csec) : 0));
+        }
+        cdef_store_row<BS, PIX>(out_fb + (size_t)(BS * by + r) * ostride + BS * bx, y, wide);
     }
 }
 
 // frame apply (svt_av1_cdef_frame, enc_cdef.c:284-600): per filter block strengths already chosen,
-// directions/variances as found by cdef_dir_kernel.  One CTA per (filter block, plane), one thread per pixel.
+// directions/variances as found by cdef_dir_kernel.  One CTA per (filter block, plane).
 template <typename PIX>
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(kT2Threads)
 cdef_apply_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const int8_t* __restrict__ fb_strength_idx,
                   const int* __restrict__ y_strength, const int* __restrict__ uv_strength, const uint8_t* __restrict__ dir_in,
                   const int* __restrict__ var_in, PIX* out_y, PIX* out_cb, PIX* out_cr, int out_stride_y, int out_stride_c) {
-    __shared__ uint16_t tile[kTileRows * kTP];
+    __shared__ __align__(16) uint16_t tile[kTileRows * kTP];
     __shared__ uint8_t  s_dir[64];
     __shared__ int      s_var[64];
     __shared__ uint8_t  s_list[64];
@@ -530,39 +659,21 @@ cdef_apply_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const
         sec = (sec + (sec == 3)) << cs;
         if (!(pri || sec)) continue;
         __syncthreads();
-        if (threadIdx.x < 64) {
-            const int  by = threadIdx.x >> 3, bx = threadIdx.x & 7, gy = fbr * 8 + by, gx = fbc * 8 + bx;
-            const bool on = gy < h8 && gx < w8 && !skip8x8[gy * w8 + gx];
-            const unsigned m = __ballot_sync(0xffffffffu, on);
-            s_dir[threadIdx.x] = dir_in[(size_t)fb * 64 + threadIdx.x];
-            s_var[threadIdx.x] = var_in[(size_t)fb * 64 + threadIdx.x];
-            if ((threadIdx.x & 31) == 0) s_ballot[threadIdx.x >> 5] = m;
-        }
-        __syncthreads();
-        const unsigned m0 = s_ballot[0], m1 = s_ballot[1];
-        const int count = __popc(m0) + __popc(m1);
+        const int count = cdef_fb_list(skip8x8, dir_in, var_in, fb, fbr, fbc, w8, h8, s_list, s_dir, s_var, s_ballot);
         if (count == 0) continue;
-        if (threadIdx.x < 64) {
-            const unsigned mine = threadIdx.x < 32 ? m0 : m1, lane = threadIdx.x & 31;
-            if ((mine >> lane) & 1) s_list[(threadIdx.x < 32 ? 0 : __popc(m0)) + __popc(mine & ((1u << lane) - 1))] = (uint8_t)threadIdx.x;
-        }
         const int dec = pli ? 1 : 0;
         const PIX* rec = (const PIX*)(pli == 0 ? f.recon_y : (pli == 1 ? f.recon_cb : f.recon_cr));
         PIX* out = pli == 0 ? out_y : (pli == 1 ? out_cb : out_cr);
         const int rstride = pli ? f.recon_stride_c : f.recon_stride_y, ostride = pli ? out_stride_c : out_stride_y;
         const int pw = f.width >> dec, ph = f.height >> dec, fbs = 64 >> dec;
         const int hsz = min(fbs, pw - fbc * fbs), vsz = min(fbs, ph - fbr * fbs);
-        stage_cdef_tile<PIX>(tile, rec, rstride, pw, ph, fbr, fbc, nvfb, nhfb, fbs, fbs, vsz, hsz);  // ends with a barrier
-        const int bsz = 8 >> dec, damping = f.damping + cs - (pli != 0);
-        for (int idx = threadIdx.x; idx < count * bsz * bsz; idx += blockDim.x) {
-            const int lg = 3 - dec, bi = idx >> (2 * lg), ri = (idx >> lg) & (bsz - 1), j = idx & (bsz - 1);
-            const int b = s_list[bi], by = b >> 3, bx = b & 7;
-            const int t = pli ? pri : cdef_adjust_strength(pri, s_var[b]);
-            const int d = pri ? s_dir[b] : 0;
-            const uint16_t* in = tile + (3 + bsz * by + ri) * kTP + 8 + bsz * bx + j;
-            out[(size_t)(fbr * fbs + bsz * by + ri) * ostride + fbc * fbs + bsz * bx + j] =
-                (PIX)cdef_filter_px(in, kTP, t, sec, d, damping, damping, cs);
-        }
+        stage_cdef_tile<PIX>(tile, rec, rstride, fbr, fbc, nvfb, nhfb, fbs, vsz, hsz);  // ends with a barrier
+        PIX* out_fb = out + (size_t)fbr * fbs * ostride + fbc * fbs;
+        const int damping = f.damping + cs - (pli != 0);
+        const size_t row_bytes = (size_t)(8 >> dec) * sizeof(PIX);  // rows start at multiples of it within a picture row
+        const bool wide = (((size_t)out | (size_t)ostride * sizeof(PIX)) & (row_bytes - 1)) == 0;
+        if (pli == 0) cdef_apply_fb<8, PIX>(tile, out_fb, ostride, wide, count, pri, sec, damping, cs, s_list, s_dir, s_var);
+        else cdef_apply_fb<4, PIX>(tile, out_fb, ostride, wide, count, pri, sec, damping, cs, s_list, s_dir, s_var);
     }
 }
 
@@ -725,12 +836,12 @@ extern "C" int svt_b200_cdef_search_frame_dev(const SvtB200CdefFrame* frame, con
     if (frame->bit_depth > 8) {
         cdef_dir_kernel<uint16_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, d_dir, d_var);
         B200_LAUNCH_CHECK();
-        cdef_search_kernel<uint16_t><<<grid_for((long long)nfb * 3, 6), 256, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
+        cdef_search_kernel<uint16_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
                                                                                 (unsigned long long*)d_mse, d_dir, d_var);
     } else {
         cdef_dir_kernel<uint8_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, d_dir, d_var);
         B200_LAUNCH_CHECK();
-        cdef_search_kernel<uint8_t><<<grid_for((long long)nfb * 3, 6), 256, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
+        cdef_search_kernel<uint8_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
                                                                                (unsigned long long*)d_mse, d_dir, d_var);
     }
     B200_LAUNCH_CHECK();
@@ -767,11 +878,11 @@ extern "C" int svt_b200_cdef_apply_frame_dev(const SvtB200CdefFrame* frame, cons
         d_var = g_cdef_var;
     }
     if (frame->bit_depth > 8)
-        cdef_apply_kernel<uint16_t><<<grid_for((long long)nfb * 3, 6), 256, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
+        cdef_apply_kernel<uint16_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
                                                                                d_dir, d_var, (uint16_t*)d_out_y, (uint16_t*)d_out_cb,
                                                                                (uint16_t*)d_out_cr, out_stride_y, out_stride_c);
     else
-        cdef_apply_kernel<uint8_t><<<grid_for((long long)nfb * 3, 6), 256, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
+        cdef_apply_kernel<uint8_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
                                                                               d_dir, d_var, (uint8_t*)d_out_y, (uint8_t*)d_out_cb,
                                                                               (uint8_t*)d_out_cr, out_stride_y, out_stride_c);
     B200_LAUNCH_CHECK();
