@@ -10,11 +10,10 @@
 //     M[k] += y[k] x, H[k][l] += y[k] y[l]; high bit depth divides by 4 / 16 at the end (truncating).
 //
 // H100 mapping of the statistics (the one dense contraction on the path):
-//   8-bit pixels -> stats_mma_kernel: exact f16 x f16 -> f32 tensor-core MMA (see the comment above it);
+//   8-bit pixels -> stats_imma_kernel: raw-pixel moments by exact u8 x u8 -> s32 tensor-core MMA, one launch per call
+//                   (see the comment above it);
 //   10/12-bit    -> the lag-sum kernels of wiener_stats_lag.cuh (H[p][q] depends only on the lag between the two samples).
-// The MMA kernel writes per-CTA int64 partials; stats_finalize_kernel adds them, mirrors the triangle and applies
-// the bit-depth divider.
-#include <cuda_fp16.h>
+#include <cooperative_groups.h>
 
 #include <map>
 
@@ -79,245 +78,296 @@ stats_sum_kernel(const PIX* __restrict__ dgd_base, const SvtB200StatsItem* __res
     if (lane == 0 && wide) atomicAdd(&tot_out[it], wide);
 }
 
-__device__ __forceinline__ int stats_average(const unsigned long long* tot, int it, const SvtB200StatsItem& s) {
-    return (int)(tot[it] / (unsigned long long)((s.h_end - s.h_start) * (s.v_end - s.v_start)));
-}
-
-constexpr int kStatsMaxParts = 32;  // CTAs cooperating on one restoration unit
-
-// partial layout per (item, part): [0, 49*49) = H (upper-triangle tiles only), [2401, 2450) = M
-//
-
 // ---------------------------------------------------------------------------------------------
-// K11, 8-bit pixels: the contraction on the tensor cores.
+// K11, 8-bit pixels: raw moments on the tensor cores, one launch per call.
 //
-// H = Y^T Y is a Gram matrix with K = pixels.  |pixel - avg| <= 255 is exact in f16, every product
-// (<= 255^2) is exact in f32 and a sum of up to 256 of them stays below 2^24, so an f16 x f16 -> f32
-// MMA chain over 256 pixels is EXACT integer arithmetic; the f32 accumulators are then converted and
-// added to int32 totals in shared memory (good for 33025 pixels), which fold into the CTA's int64
-// partial.  Bit-exact with the reference for any input; tests/test_wiener.py holds the extremes.
+// With a = find_average (the truncating mean of the region), y_k = d_k - a and x = s - a, the reference's sums follow
+// exactly, in int64, from moments of the RAW pixels:
+//     H[k][l] = sum d_k d_l - a (S_k + S_l) + N a^2          M[k] = sum d_k s - a S_k - a S_s + N a^2
+// with S_k = sum d_k (window sample k over the region), S_s = sum s and N = w h.  S_k of the centre sample is
+// find_average's own total, so nothing needs the mean before the contraction, and the Gram matrix runs on unsigned bytes:
+// mma.m16n8k32 u8 x u8 -> s32 (IMMA), exact while a warp has summed at most 33025 pixels (2^31 / 255^2).  Past that bound
+// the warps fold their int32 accumulators into the CTA's int64 totals.
 //
-// Matrix rows are ordered i = 8*kx + ky (window column kx, window row ky < WIN); row 7 is x = src - avg
-// (so M = row 7 of the same product) and rows with ky >= WIN are don't-care padding.  One
-// mma.m16n8k16 K-step covers a 2-row x 8-column block of pixels, k = 2*column + row: a fragment
-// register then holds (d[r][c], d[r+1][c]), which the tile stores pre-paired as one 32-bit word per
-// (r, c) -- any window shift is a plain word index, and with a row pitch == 4 (mod 32) words the 8
-// window rows x 4 columns a warp fetches per load land in 32 distinct banks.  The B fragment of
-// n-tile kx is also one half of the A fragment of m-tile kx/2, so a K-step costs 2*WIN loads for
-// all of its MMAs.  Only the tiles of the upper triangle (m-tile m, n-tile n >= 2m) are computed.
-constexpr int kMmaWarps = 4;
-constexpr int kMmaTW = 64, kMmaTH = 32;
-constexpr int kMmaPitch = 100;                                // words per pair-row
-constexpr int kMmaPRows = kMmaTH + 8;                         // py <= TH-2, plus window/padding row <= 8
-constexpr int kMmaXBase = kMmaPRows * kMmaPitch + 28;         // x rows sit on banks 28..31 like a window row 7
-constexpr int kMmaWords = kMmaXBase + kMmaTH * kMmaPitch;
-constexpr int kMmaAccMax = 16 * 128;                          // 16 output tiles x 128 accumulators (WIN = 7)
-constexpr int kMmaFoldPixels = 33025 - kMmaTW * kMmaTH;       // 2^31 / 255^2, minus the tile about to be added
-static_assert(kMmaPitch % 32 == 4 && (kMmaPRows * kMmaPitch) % 32 == 0, "bank layout");
-static_assert(kMmaTW + 6 <= kMmaPitch && kMmaAccMax <= 2450, "layout");
+// Matrix rows are i = 8*kx + ky (window column kx, window row ky < WIN); row 7 is x = src, row 15 (kx = 1, ky = 7) is a
+// constant 1, so the tiles (0, n) also give every S_k and S_s; the other rows with ky >= WIN are don't-care padding.  One
+// K-step covers a 4-row x 8-column block of pixels, k = 4*column + row: a fragment register then holds (d[r][c], d[r+1][c],
+// d[r+2][c], d[r+3][c]), which the tile stores as one quad word per (r, c) -- any window shift is a plain word index, and
+// with a row pitch == 4 (mod 32) words the 8 window rows x 4 columns a warp fetches per load land in 32 distinct banks.  The
+// B fragment of n-tile kx is also one half of the A fragment of m-tile kx/2, so a K-step costs 2*WIN loads for all of its
+// MMAs.  Only the tiles of the upper triangle (m-tile m, n-tile n >= 2m) are computed.  Pixels outside the region are
+// zeroed in the B operand only, so halo words may hold anything.
+//
+// A unit is one cluster of kImCluster CTAs, which share its 64x32 pixel tiles: a 256x256 luma unit gives its 8 CTAs 4
+// tiles each, a 128x128 chroma unit 1 (of 9 MMAs per K-step against 16 at 7x7).  Giving a chroma unit only 2 CTAs of 4
+// tiles, to even out the work per CTA, measured slower: the 6 idle CTAs of its cluster hold their SM slots until the
+// cluster ends, so the batch takes two waves of clusters.  Regions with fewer than 8 tiles leave the remaining CTAs
+// idle; they only take part in the cluster barriers.  The raw bytes of the next tile arrive by cp.async in a two-stage
+// ring while the current one is contracted.  The working CTAs then share the outputs: each adds the int64 totals it
+// needs over the cluster through distributed shared memory, applies the mean correction and writes M and H (both
+// triangles) in the reference layout.
+constexpr int kImWarps = 4, kImThreads = kImWarps * 32;
+constexpr int kImCluster = 8;                                  // CTAs per unit: the portable cluster size
+constexpr int kImTW = 64, kImTH = 32;
+constexpr int kImPitch = 100;                                  // words per quad-word row
+constexpr int kImQRows = kImTH + 6;                            // quad rows py + OFF + g <= TH - 4 + 9
+constexpr int kImXPitch = 80;                                  // words per src quad row (== 16 mod 32, like 4 quad rows)
+constexpr int kImXRegion = (kImQRows * kImPitch + 31) / 32 * 32;
+constexpr int kImQWords = kImXRegion + 32 + (kImTH / 4) * kImXPitch;
+constexpr int kImRawRows = kImTH + 9;                          // halo rows 0..TH+5 are loaded, the last 3 only feed padding
+constexpr int kImRawPitch = 96;                                // bytes: 70 halo columns behind a <= 15-byte alignment shift
+constexpr int kImXRawPitch = 80;                               // bytes: 64 src columns behind the shift
+constexpr int kImStage = kImRawRows * kImRawPitch + kImTH * kImXRawPitch;
+constexpr int kImAccMax = 16 * 128;                            // 16 output tiles x 128 accumulators (WIN = 7)
+constexpr int kImFoldPixels = 33025 - (kImTW * kImTH) / kImWarps;  // 2^31 / 255^2, minus what one more tile adds to a warp
+static_assert(kImPitch % 32 == 4 && kImXPitch % 32 == 16 && kImStage % 16 == 0, "bank and cp.async layout");
+// the quad builders read two words from byte (shift <= 15) + (first column of their last 4): 68 of the halo, 60 of src
+static_assert(kImTW + 8 <= kImPitch && ((15 + kImTW + 4) & ~3) + 8 <= kImRawPitch && ((15 + kImTW - 4) & ~3) + 8 <= kImXRawPitch, "layout");
 
-__device__ __forceinline__ void mma_16816_f16f32(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                                 uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+__device__ __forceinline__ void mma_16832_u8s32(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                                uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
                  : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
-
-// (lo, hi), |v| <= 255, as two f16 in one word without integer->float conversions: 0x6400 + n is the
-// f16 encoding of 1024 + n for 0 <= n < 1024, and subtracting 1280 from 1024 + (v + 256) is exact.
-__device__ __forceinline__ uint32_t pack_pair_f16(int lo, int hi) {
-    const uint32_t bits = 0x64006400u + (uint32_t)(lo + 256) + ((uint32_t)(hi + 256) << 16);
-    const __half2  h    = __hsub2(*reinterpret_cast<const __half2*>(&bits), __float2half2_rn(1280.f));
-    return *reinterpret_cast<const uint32_t*>(&h);
+__device__ __forceinline__ void cp_async16(void* dst, const void* src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async4(void* dst, const void* src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
 
 __host__ __device__ __forceinline__ int mma_tile_index(int win, int m, int n) { return m * win - m * (m - 1) + n - 2 * m; }
-// CTAs of an item that actually get pixel tiles (and so write a partial)
-__device__ __forceinline__ int stats_mma_parts(const SvtB200StatsItem& s, int ctas_per_item) {
-    const int tiles = ((s.h_end - s.h_start + kMmaTW - 1) / kMmaTW) * ((s.v_end - s.v_start + kMmaTH - 1) / kMmaTH);
-    return tiles < ctas_per_item ? tiles : ctas_per_item;
+
+// CTAs of the cluster that get pixel tiles of an item
+__device__ __forceinline__ int stats_imma_parts(const SvtB200StatsItem& s) {
+    const int tiles = ((s.h_end - s.h_start + kImTW - 1) / kImTW) * ((s.v_end - s.v_start + kImTH - 1) / kImTH);
+    return min(tiles, kImCluster);
+}
+
+// Stage rows [0, nrows) of a tile: row q starts at tile column 0 = row0 + q * stride and lands, behind its alignment
+// shift (address & 15), at dst + q * pitch.  Only rows [qlo, qhi) and tile columns [clo, chi) are read -- the rectangle
+// the reference reads -- and columns past `need` are not needed: 16-byte chunks that would cross the rectangle fall back
+// to 4-byte copies, and those to byte loads.
+__device__ __forceinline__ void stats_imma_stage_rows(uint8_t* dst, int pitch, const uint8_t* row0, ptrdiff_t stride, int nrows,
+                                                      int nchunks, int qlo, int qhi, int clo, int chi, int need) {
+    for (int w = threadIdx.x; w < nrows * nchunks; w += kImThreads) {
+        const int q = w / nchunks, ch = w - q * nchunks;
+        const uint8_t* rp = row0 + (ptrdiff_t)q * stride;
+        const int a = ch * 16 - (int)((uintptr_t)rp & 15);  // tile column of the chunk's first byte
+        if (q < qlo || q >= qhi || a >= need || a >= chi || a + 16 <= clo) continue;
+        uint8_t*       d = dst + q * pitch + ch * 16;
+        const uint8_t* g = rp + a;
+        if (a >= clo && a + 16 <= chi) {
+            cp_async16(d, g);
+            continue;
+        }
+#pragma unroll
+        for (int b4 = 0; b4 < 16; b4 += 4) {
+            if (a + b4 >= clo && a + b4 + 4 <= chi) cp_async4(d + b4, g + b4);
+            else
+                for (int b = b4; b < b4 + 4; b++)
+                    if (a + b >= clo && a + b < chi) d[b] = g[b];
+        }
+    }
+}
+
+// 4 bytes of a staged row starting at byte `at` (any alignment; the row and the word after it are in the stage)
+__device__ __forceinline__ uint32_t stats_imma_row4(const uint8_t* row, int at) {
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(row + (at & ~3));
+    return __funnelshift_r(w[0], w[1], (at & 3) * 8);
 }
 
 template <int WIN>
-__device__ __forceinline__ void stats_mma_body(const uint8_t* __restrict__ dgd, const uint8_t* __restrict__ src, const SvtB200StatsItem& s,
-                                               const int avg, const int part, const int parts, long long* __restrict__ P,
-                                               uint32_t* __restrict__ tile, int* __restrict__ s32) {
+__device__ __forceinline__ void stats_imma_body(const uint8_t* __restrict__ dgd, const uint8_t* __restrict__ src, const SvtB200StatsItem& s,
+                                                const int part, const int parts, uint32_t* __restrict__ quad, uint8_t* __restrict__ ring,
+                                                long long* __restrict__ red) {
     constexpr int NT = WIN, MT = (WIN + 1) / 2, HALF = WIN / 2, OFF = 3 - HALF;
     constexpr int NTILES = MT * WIN - MT * (MT - 1);
+    constexpr int XB = kImXRegion + ((28 + 5 * OFF) & 31);  // src quad words sit on the banks of a window row 7
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    // word offset of this lane's fragment row in n-tile n, relative to the K-step's (py, px) word
-    int boff[NT];
+    const uint32_t* lane_base = quad + (OFF + g) * kImPitch + OFF + t;  // this lane's fragment row, relative to the K-step
+    int acc[NTILES][4];
 #pragma unroll
-    for (int n = 0; n < NT; n++) boff[n] = (OFF + g) * kMmaPitch + OFF + n + t;
-    if (g == 7) boff[0] = kMmaXBase + t;
-    float acc[NTILES][4];
+    for (int i = 0; i < NTILES; i++) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0;
+    auto fold = [&]() {  // CTA-uniform: the warps add their int32 sums into the int64 totals one after another
+#pragma unroll 1
+        for (int w = 0; w < kImWarps; w++) {
+            if (warp == w)
 #pragma unroll
-    for (int i = 0; i < NTILES; i++) acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f;
-    for (int i = threadIdx.x; i < NTILES * 128; i += kMmaWarps * 32) s32[i] = 0;
-    __syncthreads();
-    auto flush_regs = [&]() {
+                for (int i = 0; i < NTILES; i++)
 #pragma unroll
-        for (int i = 0; i < NTILES; i++)
-#pragma unroll
-            for (int r = 0; r < 4; r++) {
-                atomicAdd(&s32[(i * 4 + r) * 32 + lane], __float2int_rn(acc[i][r]));
-                acc[i][r] = 0.f;
-            }
+                    for (int r = 0; r < 4; r++) {
+                        red[(i * 4 + r) * 32 + lane] += acc[i][r];
+                        acc[i][r] = 0;
+                    }
+            __syncthreads();
+        }
     };
     const int W = s.h_end - s.h_start, H = s.v_end - s.v_start;
-    const int ntx = (W + kMmaTW - 1) / kMmaTW, nty = (H + kMmaTH - 1) / kMmaTH;
-    const int vlo = s.v_start - HALF, vhi = s.v_end + HALF, hlo = s.h_start - HALF, hhi = s.h_end + HALF;
-    int  ksteps = 0, pending = 0;
-    bool spilled = false;
-    // pull the rows a tile needs towards L1 (one 128-byte line per request; every address is inside the
-    // region the reference itself reads): issued for tile k+1 right before the MMA loop of tile k
-    auto prefetch_tile = [&](int tl) {
+    const int ntx = (W + kImTW - 1) / kImTW, ntiles = ntx * ((H + kImTH - 1) / kImTH);
+    auto stage = [&](int tl, uint8_t* st) {
         const int ty = tl / ntx, tx = tl - ty * ntx;
-        const int r0 = s.v_start + ty * kMmaTH, c0 = s.h_start + tx * kMmaTW;
-        for (int w = threadIdx.x; w < 2 * (kMmaPRows + 1) + kMmaTH; w += kMmaWarps * 32) {
-            const uint8_t* p;
-            if (w < 2 * (kMmaPRows + 1)) {
-                const int row = min(max(r0 - 3 + (w >> 1), vlo), vhi - 1);
-                const int col = (w & 1) ? min(c0 + kMmaTW + 2, hhi - 1) : max(c0 - 3, hlo);
-                p = dgd + (ptrdiff_t)row * s.dgd_stride + col;
-            } else {
-                const int row = min(r0 + (w - 2 * (kMmaPRows + 1)), s.v_end - 1);
-                p = src + (ptrdiff_t)row * s.src_stride + min(c0 + 32, s.h_end - 1);
-            }
-            asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
-        }
+        const int r0 = s.v_start + ty * kImTH, c0 = s.h_start + tx * kImTW;
+        // dgd: halo rows r0-3.., columns c0-3..; the reference reads [v_start-HALF, v_end+HALF) x [h_start-HALF, h_end+HALF)
+        stats_imma_stage_rows(st, kImRawPitch, dgd + (ptrdiff_t)(r0 - 3) * s.dgd_stride + (c0 - 3), s.dgd_stride, kImTH + 6,
+                              kImRawPitch / 16, s.v_start - HALF - (r0 - 3), s.v_end + HALF - (r0 - 3), s.h_start - HALF - (c0 - 3), s.h_end + HALF - (c0 - 3),
+                              kImTW + 6);
+        // src: rows r0.., columns c0.. of the region
+        stats_imma_stage_rows(st + kImRawRows * kImRawPitch, kImXRawPitch, src + (ptrdiff_t)r0 * s.src_stride + c0, s.src_stride, kImTH,
+                              kImXRawPitch / 16, 0, s.v_end - r0, s.h_start - c0, s.h_end - c0, kImTW);
+        asm volatile("cp.async.commit_group;\n" ::: "memory");
     };
-    for (int tl = part; tl < ntx * nty; tl += parts) {
+    int pending = 0;  // pixels any one warp has added to its int32 sums
+    if (part < ntiles) stage(part, ring);
+    for (int tl = part, k = 0; tl < ntiles; tl += parts, k++) {
         const int ty = tl / ntx, tx = tl - ty * ntx;
-        const int r0 = s.v_start + ty * kMmaTH, c0 = s.h_start + tx * kMmaTW;
-        const int nrows = min(kMmaTH, s.v_end - r0), ncols = min(kMmaTW, s.h_end - c0);
-        if (pending > kMmaFoldPixels) {  // CTA-uniform: fold the int32 totals into the int64 partial
-            flush_regs();
-            ksteps = 0;
-            __syncthreads();
-            for (int i = threadIdx.x; i < NTILES * 128; i += kMmaWarps * 32) {
-                P[i] = (spilled ? P[i] : 0) + s32[i];
-                s32[i] = 0;
-            }
-            spilled = true;
-            pending = 0;
+        const int r0 = s.v_start + ty * kImTH, c0 = s.h_start + tx * kImTW;
+        const int nrows = min(kImTH, s.v_end - r0), ncols = min(kImTW, s.h_end - c0);
+        const uint8_t* st = ring + (k & 1) * kImStage;
+        if (tl + parts < ntiles) {
+            stage(tl + parts, ring + ((k + 1) & 1) * kImStage);  // the build of tile k-1 that read this stage is behind a barrier
+            asm volatile("cp.async.wait_group 1;\n" ::: "memory");
+        } else {
+            asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         }
-        __syncthreads();
-        // pair words of d = dgd - avg for tile rows/cols -3.. (zero outside what the reference reads)
-        for (int w = threadIdx.x; w < (kMmaTW + 6) * 4; w += kMmaWarps * 32) {
-            const int  seg = w / (kMmaTW + 6), c = w - seg * (kMmaTW + 6);
-            const int  col = c0 - 3 + c;
-            const bool cv = col >= hlo && col < hhi;
-            const int  rbeg = seg * (kMmaPRows / 4);
-            auto ld = [&](int rr) {
-                const int row = r0 - 3 + rr;
-                return (cv && row >= vlo && row < vhi) ? (int)dgd[(ptrdiff_t)row * s.dgd_stride + col] - avg : 0;
-            };
-            int lo = ld(rbeg);
+        __syncthreads();  // the stage is complete, and the MMAs of the previous tile are done with the quad words
+        // quad words of the halo: a thread owns 4 columns and a run of 6 quad rows, shifting one raw row in per step
+        if (threadIdx.x < 18 * 7) {
+            const int cq = (threadIdx.x % 18) * 4, q0 = (threadIdx.x / 18) * 6;
+            const uint8_t* rbase = dgd + (ptrdiff_t)(r0 - 3) * s.dgd_stride + (c0 - 3);
+            uint32_t v0 = 0, v1 = 0, v2 = 0, v3 = 0;
 #pragma unroll
-            for (int k = 0; k < kMmaPRows / 4; k++) {
-                const int hi = ld(rbeg + k + 1);
-                tile[(rbeg + k) * kMmaPitch + c] = pack_pair_f16(lo, hi);
-                lo = hi;
+            for (int j = 0; j < 9; j++) {
+                const int q = min(q0 + j, kImRawRows - 1);  // rows past the stage only feed quad rows that are not stored
+                const uint32_t b = stats_imma_row4(st + q * kImRawPitch, (int)((uintptr_t)(rbase + (ptrdiff_t)q * s.dgd_stride) & 15) + cq);
+                v0 = __byte_perm(v0, b, 0x4321);
+                v1 = __byte_perm(v1, b, 0x5321);
+                v2 = __byte_perm(v2, b, 0x6321);
+                v3 = __byte_perm(v3, b, 0x7321);
+                if (j >= 3 && q0 + j - 3 < kImQRows)
+                    *reinterpret_cast<uint4*>(quad + (q0 + j - 3) * kImPitch + cq) = make_uint4(v0, v1, v2, v3);
             }
         }
-        for (int w = threadIdx.x; w < (kMmaTH / 2) * kMmaTW; w += kMmaWarps * 32) {
-            const int  r = (w / kMmaTW) * 2, c = w % kMmaTW;
-            const bool cv = c < ncols;
-            const uint8_t* p = src + (ptrdiff_t)(r0 + r) * s.src_stride + c0 + c;
-            const int lo = (cv && r < nrows) ? (int)p[0] - avg : 0;
-            const int hi = (cv && r + 1 < nrows) ? (int)p[s.src_stride] - avg : 0;
-            tile[kMmaXBase + r * kMmaPitch + c] = pack_pair_f16(lo, hi);
+        {  // src quad words: rows 4j..4j+3 of 4 columns per thread
+            const int cq = (threadIdx.x & 15) * 4, j = threadIdx.x >> 4;
+            const uint8_t* xs = st + kImRawRows * kImRawPitch;
+            const uint8_t* rbase = src + (ptrdiff_t)r0 * s.src_stride + c0;
+            uint32_t rw[4];
+#pragma unroll
+            for (int r = 0; r < 4; r++) {
+                const int q = 4 * j + r;
+                rw[r] = stats_imma_row4(xs + q * kImXRawPitch, (int)((uintptr_t)(rbase + (ptrdiff_t)q * s.src_stride) & 15) + cq);
+            }
+            const uint32_t t0 = __byte_perm(rw[0], rw[1], 0x5140), t1 = __byte_perm(rw[0], rw[1], 0x7362);
+            const uint32_t t2 = __byte_perm(rw[2], rw[3], 0x5140), t3 = __byte_perm(rw[2], rw[3], 0x7362);
+            uint32_t* xq = quad + XB + j * kImXPitch + cq;
+            xq[0] = __byte_perm(t0, t2, 0x5410);
+            xq[1] = __byte_perm(t0, t2, 0x7632);
+            xq[2] = __byte_perm(t1, t3, 0x5410);
+            xq[3] = __byte_perm(t1, t3, 0x7632);
         }
         __syncthreads();
-        if (tl + parts < ntx * nty) prefetch_tile(tl + parts);
-        const int cgs = (ncols + 7) >> 3, nsteps = cgs * ((nrows + 1) >> 1);
-        for (int st = warp; st < nsteps; st += kMmaWarps) {
-            const int rp = st / cgs, px = (st - rp * cgs) * 8, py = rp * 2;
-            const uint32_t* base = tile + py * kMmaPitch + px;
+        const int cgs = (ncols + 7) >> 3, nsteps = cgs * ((nrows + 3) >> 2);
+        for (int stp = warp; stp < nsteps; stp += kImWarps) {
+            const int rp = stp / cgs, px = (stp - rp * cgs) * 8, py = rp * 4;
+            const uint32_t* b  = lane_base + py * kImPitch + px;
+            const uint32_t* xb = g == 7 ? quad + XB + rp * kImXPitch + px + t : b;
             // pixels of this K-step outside the region contribute nothing: zero them in the B operand
-            const uint32_t rowmask = (py + 1 < nrows) ? 0xffffffffu : 0x0000ffffu;
+            const int      nr      = nrows - py;
+            const uint32_t rowmask = nr >= 4 ? 0xffffffffu : (1u << (8 * nr)) - 1u;
             const uint32_t m0 = (px + t < ncols) ? rowmask : 0u, m1 = (px + t + 4 < ncols) ? rowmask : 0u;
             uint32_t f0[NT], f1[NT];
+            f0[0] = xb[0];
+            f1[0] = xb[4];
 #pragma unroll
-            for (int n = 0; n < NT; n++) {
-                f0[n] = base[boff[n]];
-                f1[n] = base[boff[n] + 4];
+            for (int n = 1; n < NT; n++) {
+                f0[n] = b[n];
+                f1[n] = b[n + 4];
             }
+            if (g == 7) f0[1] = f1[1] = 0x01010101u;  // row 15: the window sums
 #pragma unroll
             for (int m = 0; m < MT; m++) {
                 constexpr int last = NT - 1;
                 const int     lo = 2 * m, hi = 2 * m + 1 <= last ? 2 * m + 1 : last;
 #pragma unroll
                 for (int n = 2 * m; n < NT; n++)
-                    mma_16816_f16f32(acc[m * WIN - m * (m - 1) + n - 2 * m], f0[lo], f0[hi], f1[lo], f1[hi], f0[n] & m0, f1[n] & m1);
-            }
-            if (++ksteps == 16) {  // 256 pixels: the f32 sums are still exact integers
-                flush_regs();
-                ksteps = 0;
+                    mma_16832_u8s32(acc[m * WIN - m * (m - 1) + n - 2 * m], f0[lo], f0[hi], f1[lo], f1[hi], f0[n] & m0, f1[n] & m1);
             }
         }
-        pending += nrows * ncols;
+        pending += ((nsteps + kImWarps - 1) / kImWarps) * 32;
+        if (pending > kImFoldPixels && tl + parts < ntiles) {
+            fold();
+            pending = 0;
+        }
     }
-    flush_regs();
-    __syncthreads();
-    for (int i = threadIdx.x; i < NTILES * 128; i += kMmaWarps * 32) P[i] = (spilled ? P[i] : 0) + s32[i];
+    fold();
 }
 
-__global__ void __launch_bounds__(kMmaWarps * 32)
-stats_mma_kernel(const uint8_t* __restrict__ dgd_base, const uint8_t* __restrict__ src_base, const SvtB200StatsItem* __restrict__ items,
-                 const unsigned long long* __restrict__ tot_in, int ctas_per_item, long long* __restrict__ partial) {
-    __shared__ uint32_t tile[kMmaWords];
-    __shared__ int      s32[kMmaAccMax];
-    const int it = blockIdx.x / ctas_per_item, part = blockIdx.x % ctas_per_item;
+// grid = n_items * kImCluster CTAs, one cluster per item
+__global__ void __cluster_dims__(kImCluster, 1, 1) __launch_bounds__(kImThreads, 4)
+stats_imma_kernel(const uint8_t* __restrict__ dgd_base, const uint8_t* __restrict__ src_base, const SvtB200StatsItem* __restrict__ items,
+                  long long* __restrict__ M_out, long long* __restrict__ H_out) {
+    __shared__ __align__(16) uint32_t quad[kImQWords];
+    __shared__ __align__(16) uint8_t  ring[2 * kImStage];
+    __shared__ long long red[kImAccMax];
+    __shared__ long long sums[50];
+    namespace cgr = cooperative_groups;
+    cgr::cluster_group cluster = cgr::this_cluster();
+    const int it = blockIdx.x / kImCluster, part = (int)cluster.block_rank();
     const SvtB200StatsItem s = items[it];
-    const int avg = stats_average(tot_in, it, s);
-    if (part >= stats_mma_parts(s, ctas_per_item)) return;  // more CTAs than tiles: finalize ignores the unused partials
-    long long* P = partial + ((size_t)it * ctas_per_item + part) * 2450;
-    const uint8_t* dgd = dgd_base + s.dgd_off;
-    const uint8_t* src = src_base + s.src_off;
-    if (s.wiener_win == 7) stats_mma_body<7>(dgd, src, s, avg, part, ctas_per_item, P, tile, s32);
-    else if (s.wiener_win == 5) stats_mma_body<5>(dgd, src, s, avg, part, ctas_per_item, P, tile, s32);
-    else stats_mma_body<3>(dgd, src, s, avg, part, ctas_per_item, P, tile, s32);
-}
-
-// One thread per output element: it knows where its accumulator sits in a partial, adds that entry of
-// every part that was written, applies the bit-depth divider.  grid = (ceil(2450 / 256), n_items).
-__global__ void __launch_bounds__(256)
-stats_finalize_kernel(const long long* __restrict__ partial, int parts, const SvtB200StatsItem* __restrict__ items, int divider,
-                      int mma_layout, long long* __restrict__ M_out, long long* __restrict__ H_out) {
-    const int it = blockIdx.y, e = blockIdx.x * blockDim.x + threadIdx.x;
-    const int win = items[it].wiener_win, win2 = win * win;
-    if (e >= win2 * win2 + win2) return;
-    const int used = mma_layout ? stats_mma_parts(items[it], parts) : parts;
-    int       src;
-    if (e < win2 * win2) {
-        const int k = e / win2, l = e - k * win2;
-        int ka = k / win, kq = k - ka * win, la = l / win, lq = l - la * win;
-        if (mma_layout) {
-            // accumulator (row i = 8*kx+ky, column j) of the MMA lives in tile (i/16, j/8), C-fragment
-            // register ((i/8)&1)*2 + (j&1) of lane (i&7)*4 + (j&7)/2; only tiles with kx_i <= kx_j exist
-            if (ka > la) {
-                int x = ka; ka = la; la = x;
-                x = kq; kq = lq; lq = x;
-            }
-            src = (mma_tile_index(win, ka >> 1, la) * 4 + (ka & 1) * 2 + (lq & 1)) * 32 + kq * 4 + (lq >> 1);
-        } else {
-            // tiles were accumulated for window-column pairs a<=b only: element (k,l) lives in the
-            // tile of (k/win, l/win) when k/win <= l/win, else in its mirror
-            src = (ka <= la) ? k * win2 + l : l * win2 + k;
-        }
-    } else {
-        const int k = e - win2 * win2, ka = k / win, kq = k - ka * win;
-        src = mma_layout ? (mma_tile_index(win, 0, ka) * 4 + (kq & 1)) * 32 + 28 + (kq >> 1) : 2401 + k;  // M = matrix row 7
+    const int parts = stats_imma_parts(s), win = s.wiener_win;
+    if (part < parts) {
+        for (int i = threadIdx.x; i < kImAccMax; i += kImThreads) red[i] = 0;
+        __syncthreads();
+        const uint8_t* dgd = dgd_base + s.dgd_off;
+        const uint8_t* src = src_base + s.src_off;
+        if (win == 7) stats_imma_body<7>(dgd, src, s, part, parts, quad, ring, red);
+        else if (win == 5) stats_imma_body<5>(dgd, src, s, part, parts, quad, ring, red);
+        else stats_imma_body<3>(dgd, src, s, part, parts, quad, ring, red);
     }
-    long long v = 0;
-    for (int p = 0; p < used; p++) v += partial[((size_t)it * parts + p) * 2450 + src];
-    if (e < win2 * win2) H_out[(size_t)it * 2401 + e] = v / divider;
-    else M_out[(size_t)it * 49 + (e - win2 * win2)] = v / divider;
+    cluster.sync();  // every CTA's totals are in its shared memory
+    if (part < parts) {
+        // the working CTAs share the outputs; each adds the totals it needs over the cluster
+        // accumulator (row i = 8*kx+ky, column j) of the MMA lives in tile (i/16, j/8), C-fragment register
+        // ((i/8)&1)*2 + (j&1) of lane (i&7)*4 + (j&7)/2; only tiles with kx_i <= kx_j exist
+        auto total = [&](int idx) {
+            long long v = 0;
+#pragma unroll
+            for (int p = 0; p < kImCluster; p++)
+                if (p < parts) v += cluster.map_shared_rank(red, p)[idx];
+            return v;
+        };
+        const int win2 = win * win, half = win >> 1;
+        // row 15 (ones) x column j: S_k of window sample k = (kx, ky), and S_s in column 7
+        for (int k = threadIdx.x; k <= win2; k += kImThreads) {
+            const int kx = k / win, ky = k - kx * win;
+            sums[k] = total(k < win2 ? (mma_tile_index(win, 0, kx) * 4 + 2 + (ky & 1)) * 32 + 28 + (ky >> 1) : 3 * 32 + 31);
+        }
+        __syncthreads();
+        const long long N = (long long)(s.h_end - s.h_start) * (s.v_end - s.v_start);
+        const long long a = N ? sums[half * win + half] / N : 0, na2 = N * a * a;  // find_average
+        for (int e = part * kImThreads + threadIdx.x; e < win2 * win2 + win2; e += parts * kImThreads) {
+            if (e < win2 * win2) {
+                const int k = e / win2, l = e - k * win2;
+                int ka = k / win, kq = k - ka * win, la = l / win, lq = l - la * win;
+                if (ka > la) {
+                    int x = ka; ka = la; la = x;
+                    x = kq; kq = lq; lq = x;
+                }
+                const long long raw = total((mma_tile_index(win, ka >> 1, la) * 4 + (ka & 1) * 2 + (lq & 1)) * 32 + kq * 4 + (lq >> 1));
+                H_out[(size_t)it * 2401 + e] = raw - a * (sums[k] + sums[l]) + na2;
+            } else {
+                const int k = e - win2 * win2, ka = k / win, kq = k - ka * win;  // M = matrix row 7 (x)
+                const long long raw = total((mma_tile_index(win, 0, ka) * 4 + (kq & 1)) * 32 + 28 + (kq >> 1));
+                M_out[(size_t)it * 49 + k] = raw - a * sums[k] - a * sums[win2] + na2;
+            }
+        }
+    }
+    cluster.sync();  // no CTA leaves while another may still read its shared memory
 }
 
-// scratch of the batch call (per-CTA partials, pixel totals), one per stream: calls enqueued on
+// scratch of the 10/12-bit batch call (lag sums, pixel totals), one per stream: calls enqueued on
 // different streams may execute concurrently
 struct StatsScratch {
     long long*          acc = nullptr;
@@ -342,16 +392,16 @@ static void launch_lag_bulk(const PIX* d_dgd, const PIX* d_src, const SvtB200Sta
     B200_LAUNCH_CHECK();
 }
 
-template <typename PIX>
-static void launch_stats_mma(const PIX* d_dgd, const PIX* d_src, const SvtB200StatsItem* d_items, int n, int bd, long long* d_M,
-                             long long* d_H, long long* d_acc, unsigned long long* d_tot, cudaStream_t st);
-
-// Wiener statistics of a batch of units: 8-bit pictures on the tensor cores (stats_mma_kernel), 10 / 12 bit by lag sums
-// (wiener_stats_lag.cuh) -- both exact
+// Wiener statistics of a batch of units: 8-bit pictures on the tensor cores (stats_imma_kernel, one launch), 10 / 12 bit
+// by lag sums (wiener_stats_lag.cuh, which uses the scratch) -- both exact
 template <typename PIX>
 static void launch_stats(const PIX* d_dgd, const PIX* d_src, const SvtB200StatsItem* d_items, int n, int bd, long long* d_M,
                          long long* d_H, long long* d_acc, unsigned long long* d_tot, cudaStream_t st) {
-    if constexpr (sizeof(PIX) == 1) return launch_stats_mma<PIX>(d_dgd, d_src, d_items, n, bd, d_M, d_H, d_acc, d_tot, st);
+    if constexpr (sizeof(PIX) == 1) {
+        stats_imma_kernel<<<n * kImCluster, kImThreads, 0, st>>>(d_dgd, d_src, d_items, d_M, d_H);
+        B200_LAUNCH_CHECK();
+        return;
+    }
     const int divider = bd == 12 ? 16 : (bd == 10 ? 4 : 1);
     int cpi = (ctx().sm_count * 8) / (n > 0 ? n : 1);  // CTAs per unit: ~8 resident CTAs per SM over the batch
     if (cpi < 1) cpi = 1;
@@ -372,24 +422,6 @@ static void launch_stats(const PIX* d_dgd, const PIX* d_src, const SvtB200StatsI
 }
 
 template <typename PIX>
-static void launch_stats_mma(const PIX* d_dgd, const PIX* d_src, const SvtB200StatsItem* d_items, int n, int bd, long long* d_M,
-                             long long* d_H, long long* d_acc, unsigned long long* d_tot, cudaStream_t st) {
-    const int divider = bd == 12 ? 16 : (bd == 10 ? 4 : 1);
-    // CTAs per item: enough for ~6 resident CTAs per SM (the tensor-core kernel gives each of them 1-2 pixel tiles)
-    int cpi = (ctx().sm_count * (sizeof(PIX) == 1 ? 6 : 4)) / (n > 0 ? n : 1);
-    if (cpi < 1) cpi = 1;
-    if (cpi > (sizeof(PIX) == 1 ? kStatsMaxParts : 16)) cpi = sizeof(PIX) == 1 ? kStatsMaxParts : 16;
-    B200_CUDA_CHECK(cudaMemsetAsync(d_tot, 0, (size_t)n * sizeof(unsigned long long), st));
-    stats_sum_kernel<PIX><<<n * kSumParts, 256, 0, st>>>(d_dgd, d_items, d_tot);
-    B200_LAUNCH_CHECK();
-    static_assert(sizeof(PIX) == 1, "the tensor-core statistics are the 8-bit path (high bit depth: wiener_stats_lag.cuh)");
-    stats_mma_kernel<<<n * cpi, kMmaWarps * 32, 0, st>>>(d_dgd, d_src, d_items, d_tot, cpi, d_acc);
-    B200_LAUNCH_CHECK();
-    stats_finalize_kernel<<<dim3((2450 + 255) / 256, n), 256, 0, st>>>(d_acc, cpi, d_items, divider, sizeof(PIX) == 1, d_M, d_H);
-    B200_LAUNCH_CHECK();
-}
-
-template <typename PIX>
 static void stats_t1(int wiener_win, const PIX* dgd, const PIX* src, int h_start, int h_end, int v_start, int v_end, int dgd_stride,
                      int src_stride, int64_t* M, int64_t* H, int bd) {
     require_ready();
@@ -399,7 +431,7 @@ static void stats_t1(int wiener_win, const PIX* dgd, const PIX* src, int h_start
     LaneGuard l;
     size_t o_d = l->alloc((size_t)dw * dh * sizeof(PIX)), o_s = l->alloc((size_t)w * h * sizeof(PIX)), o_it = l->alloc(sizeof(SvtB200StatsItem));
     size_t in_end = l->used;
-    size_t o_M = l->alloc(49 * 8), o_H = l->alloc(2401 * 8), o_acc = l->alloc((size_t)kStatsMaxParts * 2450 * 8), o_avg = l->alloc(16);
+    size_t o_M = l->alloc(49 * 8), o_H = l->alloc(2401 * 8), o_acc = l->alloc((size_t)kLagItemWords * 8), o_avg = l->alloc(16);
     for (int r = 0; r < dh; r++)
         memcpy(l->h<PIX>(o_d) + (size_t)r * dw, dgd + (ptrdiff_t)(v_start - half + r) * dgd_stride + h_start - half, dw * sizeof(PIX));
     for (int r = 0; r < h; r++) memcpy(l->h<PIX>(o_s) + (size_t)r * w, src + (ptrdiff_t)(v_start + r) * src_stride + h_start, w * sizeof(PIX));
@@ -494,18 +526,19 @@ extern "C" int svt_b200_compute_stats_batch_dev(const void* d_dgd, const void* d
                                                 int bit_depth, int64_t* d_M, int64_t* d_H, void* stream) {
     require_ready();
     if (n_items <= 0) return n_items == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
+    if (bit_depth <= 8) {
+        launch_stats<uint8_t>((const uint8_t*)d_dgd, (const uint8_t*)d_src, d_items, n_items, 8, (long long*)d_M, (long long*)d_H, nullptr,
+                              nullptr, (cudaStream_t)stream);
+        return SVT_B200_OK;
+    }
     std::lock_guard<std::mutex> lk(g_stats_mu);
     StatsScratch& sc = g_stats[(cudaStream_t)stream];
     if ((size_t)n_items > sc.cap) {
         sc.cap = (size_t)n_items * 2;  // new buffers; the old ones live on until shutdown (captured graphs may replay them)
-        sc.acc = (long long*)scratch_alloc(sc.cap * kStatsMaxParts * 2450 * 8);
+        sc.acc = (long long*)scratch_alloc(sc.cap * kLagItemWords * 8);
         sc.tot = (unsigned long long*)scratch_alloc(sc.cap * 8);
     }
-    if (bit_depth > 8)
-        launch_stats<uint16_t>((const uint16_t*)d_dgd, (const uint16_t*)d_src, d_items, n_items, bit_depth, (long long*)d_M, (long long*)d_H,
-                               sc.acc, sc.tot, (cudaStream_t)stream);
-    else
-        launch_stats<uint8_t>((const uint8_t*)d_dgd, (const uint8_t*)d_src, d_items, n_items, 8, (long long*)d_M, (long long*)d_H, sc.acc,
-                              sc.tot, (cudaStream_t)stream);
+    launch_stats<uint16_t>((const uint16_t*)d_dgd, (const uint16_t*)d_src, d_items, n_items, bit_depth, (long long*)d_M, (long long*)d_H,
+                           sc.acc, sc.tot, (cudaStream_t)stream);
     return SVT_B200_OK;
 }

@@ -12,10 +12,10 @@
 // with RAW pixels (no mean removed: products are non-negative, 8-bit pictures take four multiply-accumulates per DP4A) and
 // the mean folded back in at the end:  sum (y-a)(z-a) = sum yz - a (sum y + sum z) + N a^2  (a = the integer average).
 // That is (2 win - 1) win - (win - 1) = 85 lags + 49 cross lags for M per pixel instead of 1274, identical results, same code for
-// 8 / 10 / 12 bit.  Measured (1080p, ncu): the 8-bit form still costs more instructions than the exact-f16 tensor-core Gram
-// matrix (57 M vs 31 M warp instructions per picture -- the partner extraction dominates), so 8-bit pictures stay on
-// stats_mma_kernel; for 10 / 12 bit, where no exact tensor-core form exists, it replaces the 49-MAC-per-pixel integer kernel
-// and halves the call.
+// 8 / 10 / 12 bit.  Measured on the previous target GPU (1080p, ncu): the 8-bit form cost more instructions than the
+// tensor-core Gram matrix of that time (57 M vs 31 M warp instructions per picture -- the partner extraction dominates), so
+// 8-bit pictures use the tensor cores (stats_imma_kernel, wiener.cu); for 10 / 12 bit, where no exact tensor-core form
+// exists, it replaces the 49-MAC-per-pixel integer kernel and halves the call.
 //
 //   stats_lag_bulk_kernel   CC of every lag, sum x Y(shift) for M, plain pixel sums: one CTA per (8-row band, unit); warp g owns
 //                           the lags with dy = g and the M shifts with lr = g - half; partner words come from a 5 / 7 word

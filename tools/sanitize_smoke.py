@@ -12,7 +12,7 @@ from svt_av1_psy_b200.pipeline import FramePipeline  # noqa: E402
 from svt_av1_psy_b200.workload import FrameWorkload  # noqa: E402
 
 pkg.init(0)
-for bd in (8, 10):  # 8-bit: HMMA statistics, u8 TMA maps; 10-bit: lag-sum statistics, u16 planes
+for bd in (8, 10):  # 8-bit: IMMA statistics, u8 TMA maps; 10-bit: lag-sum statistics, u16 planes
     fp = FramePipeline(FrameWorkload(384, 256, bit_depth=bd), torch)
     fp.load_inputs()
     fp.step()
