@@ -444,7 +444,10 @@ SVT_B200_API uint64_t svt_b200_search_one_dual(int* lev0, int* lev1, int nb_stre
 /* T2: whole-picture CDEF strength search (cdef_seg_search, cdef_process.c:106-352) and apply
  * (svt_av1_cdef_frame, enc_cdef.c:284).  4:2:0, width/height multiples of 8, all pointers DEVICE
  * memory pointing at the first visible pixel of each plane.  recon_* = deblocked reconstruction
- * (filter input), src_* = source picture.  Pixels are uint8 (bit_depth 8) or uint16. */
+ * (filter input), src_* = source picture.  Pixels are uint8 (bit_depth 8) or uint16.  Like the
+ * reference, both calls read recon_cb / recon_cr rows up to 4 pixels past the chroma width when the last
+ * filter block column is 8 luma pixels wide (the 8-pixel right border of its neighbour's tile): those
+ * pixels never change the result, but they must be readable memory. */
 typedef struct SvtB200CdefFrame {
     const void* recon_y; const void* recon_cb; const void* recon_cr;
     const void* src_y;   const void* src_cb;   const void* src_cr;

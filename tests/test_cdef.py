@@ -75,6 +75,20 @@ def test_compute_cdef_dist_t1(b200, refc):
                         assert a == b
 
 
+def test_copy_rect8_8bit_to_16bit_t1(b200, refc):
+    """every size from 1x1 to 64x64 at odd strides; nothing outside the v x h rectangle is written"""
+    r = rng(74)
+    f = refc.svt_aom_copy_rect8_8bit_to_16bit_c; f.restype = None
+    for v in range(1, 65):
+        for h in range(1, 65):
+            ss, ds = (h | 1) + 2 * int(r.integers(0, 4)), (h | 1) + 2 * int(r.integers(1, 4))
+            src = r.integers(0, 256, v * ss, dtype=np.uint8)
+            a = np.full(v * ds + 8, 0xabcd, np.uint16); b = a.copy()
+            f(ch.P(a), ds, ch.P(src), ss, v, h)
+            b200.lib.svt_b200_aom_copy_rect8_8bit_to_16bit(ch.P(b), ds, ch.P(src), ss, v, h)
+            assert np.array_equal(a, b), (v, h, ss, ds)
+
+
 def test_search_one_dual_t1(b200, refc):
     r = rng(72)
     f = refc.svt_search_one_dual_c; f.restype = ct.c_uint64

@@ -133,6 +133,35 @@ def test_port_cdef_search_matches_reference(oracle, refc, bd, subs):
     assert np.array_equal(a[0], b[0])
 
 
+@pytest.mark.parametrize("bd", [8, 10, 12])
+def test_cdef_apply_replay_matches_ref_driver(refc, bd):
+    """cdef_helpers.ref_cdef_apply (the checker of the GPU apply) == ref_cdef_apply_frame of oracle/ref_driver.c (the
+    producer of the committed goldens): every strength code in both planes, dampings 3..6, untouched (-1) and partial
+    filter blocks, output planes whose pitch is not their width"""
+    r = rng(150 + bd)
+    dt = np.uint8 if bd == 8 else np.uint16
+    perm = [int(c) for c in r.permutation(64)]
+    changed = [False] * 3
+    for i, ((W, H), damping) in enumerate(zip([(8, 8), (72, 72), (200, 136), (456, 264)], (3, 4, 5, 6))):
+        rec, _, skip = ch.make_mixed_frame(r, W, H, bd)
+        nfb = ((W + 63) // 64) * ((H + 63) // 64)
+        sy, su = (perm * 2)[16 * i:16 * i + 16], (perm * 2)[16 * i + 7:16 * i + 23]
+        sy[3] = su[3] = 0
+        idx = r.integers(-1, 16, nfb).astype(np.int8)
+        outs = []
+        for fn in (ch.ref_cdef_apply, ch.c_cdef_apply):
+            pitch = [W + 5, (W >> 1) + 3, (W >> 1) + 3]
+            bufs = [np.full((p.shape[0], s), 0xa5, dt) for p, s in zip(rec, pitch)]
+            for b, p in zip(bufs, rec):
+                b[:, :p.shape[1]] = p
+            fn(refc, rec, skip, W, H, bd, damping, idx, sy, su, bufs, pitch)
+            outs.append(bufs)
+        for pli in range(3):
+            assert np.array_equal(outs[0][pli], outs[1][pli]), (W, H, pli)
+            changed[pli] |= not np.array_equal(outs[0][pli][:, :rec[pli].shape[1]], rec[pli])
+    assert all(changed), "every plane must have been filtered somewhere"
+
+
 # ---- Wiener --------------------------------------------------------------------------------------
 import rest_helpers as rh  # noqa: E402
 
