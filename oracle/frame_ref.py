@@ -6,25 +6,18 @@ ref_frames_run take).  Nothing here imports the product package: the workload mo
 stand-alone (pure numpy), so a process that only times the CPU arm never maps libsvtav1_b200.so.
 """
 import ctypes as ct
-import importlib
-import os
 import sys
 
 import numpy as np
 
 from . import support as me_np
 
-_PKG = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "svt-av1-psy_b200")
 vp = ct.c_void_p
 
 
 def load_workload_module():
-    """svt-av1-psy_b200/workload.py + layout.py as top-level modules (no package __init__, no .so)"""
-    if "svt_av1_psy_b200.workload" in sys.modules:  # the product package is already imported (tests, H100 arm)
-        return sys.modules["svt_av1_psy_b200.workload"]
-    if _PKG not in sys.path:
-        sys.path.append(_PKG)
-    return importlib.import_module("workload")
+    """svt-av1-psy_b200/workload.py, loaded without libsvtav1_b200.so unless the product package is already imported"""
+    return me_np.load_pkg_module("workload")
 
 
 class RefFrameJob(ct.Structure):
@@ -83,7 +76,7 @@ class RefFrame:
         self.cur_pyr = me_np.build_pyramid_np(wl.me_luma(wl.cur), W, H, wl.me_shapes)
         self.ref_pyrs = [me_np.build_pyramid_np(wl.me_luma(r), W, H, wl.me_shapes) for r in wl.refs]
         self.cur_desc = me_np.ref_pic_desc(self.cur_pyr, wl.me_shapes)
-        self.ref_descs = (me_np.RefMePicture * wl.n_refs)(*[me_np.ref_pic_desc(p, wl.me_shapes) for p in self.ref_pyrs])
+        self.ref_descs = (me_np.MePicture * wl.n_refs)(*[me_np.ref_pic_desc(p, wl.me_shapes) for p in self.ref_pyrs])
         self.me_cfg = me_cfg_for(wl)
         nb = ((W + 63) // 64) * ((H + 63) // 64)
         mc, mr, n_pu = wl.me_controls["max_cand"], wl.me_controls["max_refs"], wl.me_n_pu

@@ -27,6 +27,7 @@
 #include "restoration.h"
 #include "convolve.h"
 #include "inv_transforms.h"
+#include "../include/svt_b200.h" /* the T2 work items and picture descriptors the drivers below take */
 
 
 /* ---- persistent, core-pinned worker pool -------------------------------------------------------------
@@ -214,8 +215,7 @@ int ref_set_tier(int avx2) {
  * restates hme_level_0/1/2 (motion_estimation.c:820-1113), set_final_seach_centre_sb (:2182-2390),
  * check_00_center (:1139-1210), integer_search_b64 (:1249-1520), open_loop_me_fullpel_search_sblock
  * (:781-817) for the controls the H100 T2 path honours (see DESIGN.md). */
-#include "ref_me_b64.h" /* RefMePicture + the complete driver (ref_me_b64.c) */
-typedef struct { int32_t hme_l0_sa_w, hme_l0_sa_h, hme_l1_sa_w, hme_l1_sa_h, hme_l2_sa_w, hme_l2_sa_h, me_sa_w, me_sa_h, hme_sub_sad, me_sub_sad, check_zero_centre, reserved; } RefMeParams;
+#include "ref_me_b64.h" /* the complete driver (ref_me_b64.c) */
 
 static void hme_clip(int16_t org, int16_t* origin, int16_t* sa, int16_t pad, int16_t pic, int round8) {
     if ((int16_t)(org + *origin) < -pad) {
@@ -257,12 +257,12 @@ static void fullpel_b64(const uint8_t* src, uint32_t ss, const uint8_t* ref, uin
     }
 }
 
-typedef struct { const RefMePicture* cur; const RefMePicture* refs; const RefMeParams* prm; int n_refs; uint32_t* best_sad; uint32_t* best_mv; int16_t* hme_centre; uint64_t* hme_sad; } MeCtx;
+typedef struct { const SvtB200MePicture* cur; const SvtB200MePicture* refs; const SvtB200MeParams* prm; int n_refs; uint32_t* best_sad; uint32_t* best_mv; int16_t* hme_centre; uint64_t* hme_sad; } MeCtx;
 static void ref_me_picture_body(void* vctx, int i) {
     const MeCtx* c = (const MeCtx*)vctx;
-    const RefMePicture* cur = c->cur;
-    const RefMePicture* refs = c->refs;
-    const RefMeParams* prm = c->prm;
+    const SvtB200MePicture* cur = c->cur;
+    const SvtB200MePicture* refs = c->refs;
+    const SvtB200MeParams* prm = c->prm;
     uint32_t* best_sad = c->best_sad;
     uint32_t* best_mv = c->best_mv;
     int16_t* hme_centre = c->hme_centre;
@@ -270,8 +270,8 @@ static void ref_me_picture_body(void* vctx, int i) {
     const int W = cur->width[2], H = cur->height[2], b64_w = (W + 63) >> 6, b64_h = (H + 63) >> 6, nb = b64_w * b64_h;
     {
         const int r = i / nb, b = i % nb, bx = b % b64_w, by = b / b64_w;
-        const RefMePicture* rp = &refs[r];
-        const RefMeParams*  p  = &prm[r];
+        const SvtB200MePicture* rp = &refs[r];
+        const SvtB200MeParams*  p  = &prm[r];
         const int sub = p->hme_sub_sad ? 1 : 0;
         int16_t  px[4] = {0, 0, 0, 0}, py[4] = {0, 0, 0, 0};
         uint64_t ls[4] = {0, 0, 0, 0};
@@ -350,7 +350,7 @@ static void ref_me_picture_body(void* vctx, int i) {
                     best_mv + (size_t)i * 85);
         }
 }
-void ref_me_picture(const RefMePicture* cur, const RefMePicture* refs, const RefMeParams* prm, int n_refs, uint32_t* best_sad,
+void ref_me_picture(const SvtB200MePicture* cur, const SvtB200MePicture* refs, const SvtB200MeParams* prm, int n_refs, uint32_t* best_sad,
                     uint32_t* best_mv, int16_t* hme_centre, uint64_t* hme_sad) {
     MeCtx c = {cur, refs, prm, n_refs, best_sad, best_mv, hme_centre, hme_sad};
     const int W = cur->width[2], H = cur->height[2], b64_w = (W + 63) >> 6, b64_h = (H + 63) >> 6, nb = b64_w * b64_h;
@@ -362,12 +362,6 @@ void ref_me_picture(const RefMePicture* cur, const RefMePicture* refs, const Ref
  * the trio of svt_aom_estimate_transform -> svt_aom_quantize_inv_quantize -> inverse (SURVEY 3.4),
  * one call per block; 8-bit or 10-bit pixels (the reference's CONVERT_TO_BYTEPTR disguise for 16-bit
  * planes, full_loop.c:1843-1846), "fp" quantizer with quantisation matrices (PSY default). */
-typedef struct { uint64_t src_off, dst_off; uint32_t src_stride; uint8_t tx_size, tx_type; uint16_t reserved; } RefFwdItem;
-typedef struct { uint64_t coef_off, pred_off, recon_off; uint32_t pred_stride, recon_stride; uint8_t tx_size, tx_type, bd, reserved; uint32_t reserved2; } RefInvItem;
-typedef struct {
-    uint64_t coeff_off, q_off, dq_off; uint32_t scan_off, qm_off, iqm_off, n_coeffs;
-    int16_t zbin[2], round[2], quant[2], quant_shift[2], dequant[2]; uint8_t mode, log_scale; uint16_t reserved;
-} RefQuantItem;
 static const int TXW[19] = {4, 8, 16, 32, 64, 4, 8, 8, 16, 16, 32, 32, 64, 4, 16, 8, 32, 16, 64};
 static const int TXH[19] = {4, 8, 16, 32, 64, 8, 4, 16, 8, 32, 16, 64, 32, 16, 4, 32, 8, 64, 16};
 
@@ -397,7 +391,7 @@ static void fwd_one(int16_t* in, int32_t* out, uint32_t stride, int ty, int sz, 
 
 typedef struct {
     const int16_t* residual; int32_t *coeff, *q, *dq; const int16_t *scan, *iscan; const uint8_t* qm;
-    const RefFwdItem* fwd; const RefQuantItem* qi; const RefInvItem* inv; uint16_t* eobs;
+    const SvtB200FwdTxfmItem* fwd; const SvtB200QuantItem* qi; const SvtB200InvTxfmItem* inv; uint16_t* eobs;
     const void* pred; void* recon; int bd;
     const void* srcpix; int16_t* residual_w; int skip_zero_blocks;
 } TxCtx;
@@ -405,8 +399,8 @@ typedef struct {
 /* svt_aom_residual_kernel (coding_loop.c:69, called per transform block at :393,:471,:518): residual = source - prediction */
 static void residual_body(void* vctx, int i) {
     const TxCtx* c = (const TxCtx*)vctx;
-    const RefFwdItem* it = &c->fwd[i];
-    const RefInvItem* iv = &c->inv[i];
+    const SvtB200FwdTxfmItem* it = &c->fwd[i];
+    const SvtB200InvTxfmItem* iv = &c->inv[i];
     const int W = TXW[it->tx_size], H = TXH[it->tx_size];
     if (c->bd == 8)
         svt_residual_kernel8bit((uint8_t*)c->srcpix + it->src_off, it->src_stride, (uint8_t*)c->pred + iv->pred_off, iv->pred_stride,
@@ -418,7 +412,7 @@ static void residual_body(void* vctx, int i) {
 
 static void fwd_body(void* vctx, int i) {
     const TxCtx* c = (const TxCtx*)vctx;
-    const RefFwdItem* it = &c->fwd[i];
+    const SvtB200FwdTxfmItem* it = &c->fwd[i];
     const int W = TXW[it->tx_size], H = TXH[it->tx_size];
     if ((it->reserved & 1) && (W > 32 || H > 32)) {
         /* packed output: the re-pack half of svt_handle_transform64x64 & co (transforms.c:2374-2542) */
@@ -430,20 +424,20 @@ static void fwd_body(void* vctx, int i) {
     }
     fwd_one((int16_t*)c->residual + it->src_off, c->coeff + it->dst_off, it->src_stride, it->tx_type, it->tx_size, c->bd);
 }
-void ref_fwd_txfm_batch_bd(const int16_t* residual, int32_t* coeff, const RefFwdItem* items, int n, int bd) {
+void ref_fwd_txfm_batch_bd(const int16_t* residual, int32_t* coeff, const SvtB200FwdTxfmItem* items, int n, int bd) {
     TxCtx c;
     memset(&c, 0, sizeof(c));
     c.residual = residual; c.coeff = coeff; c.fwd = items; c.bd = bd;
     par_for(n, 64, fwd_body, &c);
 }
-void ref_fwd_txfm_batch(const int16_t* residual, int32_t* coeff, const RefFwdItem* items, int n) { ref_fwd_txfm_batch_bd(residual, coeff, items, n, 8); }
+void ref_fwd_txfm_batch(const int16_t* residual, int32_t* coeff, const SvtB200FwdTxfmItem* items, int n) { ref_fwd_txfm_batch_bd(residual, coeff, items, n, 8); }
 
 static void quant_body(void* vctx, int i) {
     const TxCtx* c = (const TxCtx*)vctx;
     const int32_t* coeff = c->coeff;
     int32_t *q = c->q, *dq = c->dq;
     uint16_t* eobs = c->eobs;
-    const RefQuantItem* it = &c->qi[i];
+    const SvtB200QuantItem* it = &c->qi[i];
     const uint8_t* wm = it->qm_off == 0xffffffffu ? NULL : c->qm + it->qm_off;
     const uint8_t* im = it->iqm_off == 0xffffffffu ? NULL : c->qm + it->iqm_off;
     const int16_t* sc = c->scan + it->scan_off;
@@ -485,7 +479,7 @@ static void quant_body(void* vctx, int i) {
                                    dq + it->dq_off, dequant, &eobs[i], sc, isc, it->log_scale);
 }
 void ref_quant_batch(const int32_t* coeff, int32_t* q, int32_t* dq, const int16_t* scan, const int16_t* iscan, const uint8_t* qm,
-                     const RefQuantItem* items, int n, uint16_t* eobs) {
+                     const SvtB200QuantItem* items, int n, uint16_t* eobs) {
     TxCtx c;
     memset(&c, 0, sizeof(c));
     c.coeff = (int32_t*)coeff; c.q = q; c.dq = dq; c.scan = scan; c.iscan = iscan; c.qm = qm; c.qi = items; c.eobs = eobs;
@@ -496,7 +490,7 @@ void ref_quant_batch(const int32_t* coeff, int32_t* q, int32_t* dq, const int16_
  * wrappers; read and write planes differ, so they pass the maximum eob themselves */
 static void inv_body(void* vctx, int i) {
     const TxCtx* c = (const TxCtx*)vctx;
-    const RefInvItem* it = &c->inv[i];
+    const SvtB200InvTxfmItem* it = &c->inv[i];
     if (c->skip_zero_blocks && c->eobs[i] == 0) {
         /* no coefficient survived: the encode pass does not run the inverse (coding_loop.c:601,632,655), the
          * reconstruction is the prediction */
@@ -515,21 +509,17 @@ static void inv_body(void* vctx, int i) {
                                     CONVERT_TO_BYTEPTR((uint16_t*)c->recon + it->recon_off), it->recon_stride, (TxSize)it->tx_size,
                                     (uint32_t)c->bd, (TxType)it->tx_type, PLANE_TYPE_Y, 0, 0);
 }
-void ref_inv_txfm_batch_bd(const int32_t* coeff, const void* pred, void* recon, const RefInvItem* items, int n, int bd) {
+void ref_inv_txfm_batch_bd(const int32_t* coeff, const void* pred, void* recon, const SvtB200InvTxfmItem* items, int n, int bd) {
     TxCtx c;
     memset(&c, 0, sizeof(c));
     c.dq = (int32_t*)coeff; c.pred = pred; c.recon = recon; c.inv = items; c.bd = bd;
     par_for(n, 64, inv_body, &c);
 }
-void ref_inv_txfm_batch_8bit(const int32_t* coeff, const uint8_t* pred, uint8_t* recon, const RefInvItem* items, int n) {
+void ref_inv_txfm_batch_8bit(const int32_t* coeff, const uint8_t* pred, uint8_t* recon, const SvtB200InvTxfmItem* items, int n) {
     ref_inv_txfm_batch_bd(coeff, pred, recon, items, n, 8);
 }
 
 /* ---- CDEF picture search / apply (cdef_seg_search, cdef_process.c:106-352; svt_av1_cdef_frame) ----- */
-typedef struct {
-    const void *recon_y, *recon_cb, *recon_cr, *src_y, *src_cb, *src_cr;
-    int32_t recon_stride_y, recon_stride_c, src_stride_y, src_stride_c, width, height, bit_depth, damping, subsampling_factor, reserved;
-} RefCdefFrame;
 
 static void cdef_tile(uint16_t* inbuf, const void* plane, int stride, int fbr, int fbc, int nvfb, int nhfb, int fbs, int vsz, int hsz, int is16) {
     uint16_t* in = inbuf + CDEF_VBORDER * CDEF_BSTRIDE + CDEF_HBORDER;
@@ -539,7 +529,7 @@ static void cdef_tile(uint16_t* inbuf, const void* plane, int stride, int fbr, i
     svt_aom_copy_sb8_16(&in[-yoff * CDEF_BSTRIDE - xoff], CDEF_BSTRIDE, (const uint8_t*)plane, fbr * fbs - yoff, fbc * fbs - xoff, stride, ysize, xsize,
                         is16 ? true : false);
 }
-static int cdef_list(const RefCdefFrame* f, const uint8_t* skip8x8, int fbr, int fbc, CdefList* dlist) {
+static int cdef_list(const SvtB200CdefFrame* f, const uint8_t* skip8x8, int fbr, int fbc, CdefList* dlist) {
     const int w8 = (f->width + 7) >> 3, h8 = (f->height + 7) >> 3;
     int cnt = 0;
     for (int by = 0; by < 8; by++)
@@ -550,10 +540,10 @@ static int cdef_list(const RefCdefFrame* f, const uint8_t* skip8x8, int fbr, int
     return cnt;
 }
 
-typedef struct { const RefCdefFrame* f; const uint8_t* skip; const int *sy, *su; int ng; uint64_t* mse; uint8_t* dir; int32_t* var; } CdefSearchCtx;
+typedef struct { const SvtB200CdefFrame* f; const uint8_t* skip; const int *sy, *su; int ng; uint64_t* mse; uint8_t* dir; int32_t* var; } CdefSearchCtx;
 static void cdef_search_body(void* vctx, int fb) {
     const CdefSearchCtx* c = (const CdefSearchCtx*)vctx;
-    const RefCdefFrame* f = c->f;
+    const SvtB200CdefFrame* f = c->f;
     const int ng = c->ng;
     uint64_t* mse = c->mse;
     const int is16 = f->bit_depth > 8, coeff_shift = f->bit_depth - 8, psz = is16 ? 2 : 1;
@@ -601,16 +591,16 @@ static void cdef_search_body(void* vctx, int fb) {
         c->var[(size_t)fb * 64 + dlist[k].by * 8 + dlist[k].bx] = var[dlist[k].by][dlist[k].bx];
     }
 }
-void ref_cdef_search_frame(const RefCdefFrame* f, const uint8_t* skip8x8, const int* str_y, const int* str_uv, int ng, uint64_t* mse, uint8_t* dir_out,
+void ref_cdef_search_frame(const SvtB200CdefFrame* f, const uint8_t* skip8x8, const int* str_y, const int* str_uv, int ng, uint64_t* mse, uint8_t* dir_out,
                            int32_t* var_out) {
     CdefSearchCtx c = {f, skip8x8, str_y, str_uv, ng, mse, dir_out, var_out};
     par_for(((f->width + 63) >> 6) * ((f->height + 63) >> 6), 2, cdef_search_body, &c);
 }
 
-typedef struct { const RefCdefFrame* f; const uint8_t* skip; const int8_t* idx; const int *ys, *us; void *oy, *ocb, *ocr; int os_y, os_c; } CdefApplyCtx;
+typedef struct { const SvtB200CdefFrame* f; const uint8_t* skip; const int8_t* idx; const int *ys, *us; void *oy, *ocb, *ocr; int os_y, os_c; } CdefApplyCtx;
 static void cdef_apply_body(void* vctx, int fb) {
     const CdefApplyCtx* c = (const CdefApplyCtx*)vctx;
-    const RefCdefFrame* f = c->f;
+    const SvtB200CdefFrame* f = c->f;
     const int is16 = f->bit_depth > 8, coeff_shift = f->bit_depth - 8;
     const int nhfb = (f->width + 63) >> 6, nvfb = (f->height + 63) >> 6;
     const int fbr = fb / nhfb, fbc = fb % nhfb;
@@ -639,22 +629,20 @@ static void cdef_apply_body(void* vctx, int fb) {
                                pri, sec + (sec == 3), f->damping, f->damping, coeff_shift, 1);
     }
 }
-void ref_cdef_apply_frame(const RefCdefFrame* f, const uint8_t* skip8x8, const int8_t* fb_idx, const int* y_str, const int* uv_str, void* out_y,
+void ref_cdef_apply_frame(const SvtB200CdefFrame* f, const uint8_t* skip8x8, const int8_t* fb_idx, const int* y_str, const int* uv_str, void* out_y,
                           void* out_cb, void* out_cr, int os_y, int os_c) {
     CdefApplyCtx c = {f, skip8x8, fb_idx, y_str, uv_str, out_y, out_cb, out_cr, os_y, os_c};
     par_for(((f->width + 63) >> 6) * ((f->height + 63) >> 6), 2, cdef_apply_body, &c);
 }
 
 /* ---- Wiener statistics / filter over unit lists ------------------------------------------------------ */
-typedef struct { uint64_t dgd_off, src_off; int32_t dgd_stride, src_stride, h_start, h_end, v_start, v_end, wiener_win, reserved; } RefStatsItem;
-typedef struct { uint64_t src_off, dst_off; int32_t src_stride, dst_stride; uint16_t w, h; uint32_t reserved; int16_t hfilter[8], vfilter[8]; } RefWienerUnit;
 
-typedef struct { const void *dgd, *src; const RefStatsItem* items; int64_t *M, *H; int bd; } StatsCtx;
+typedef struct { const void *dgd, *src; const SvtB200StatsItem* items; int64_t *M, *H; int bd; } StatsCtx;
 static void stats_body(void* vctx, int i) {
     const StatsCtx* c = (const StatsCtx*)vctx;
     DECLARE_ALIGNED(64, int64_t, m[WIENER_WIN2 + 7]);
     DECLARE_ALIGNED(64, int64_t, h[WIENER_WIN2 * WIENER_WIN2 + 7]);
-    const RefStatsItem* it = &c->items[i];
+    const SvtB200StatsItem* it = &c->items[i];
     if (c->bd == 8)
         svt_av1_compute_stats(it->wiener_win, (const uint8_t*)c->dgd + it->dgd_off, (const uint8_t*)c->src + it->src_off, it->h_start, it->h_end,
                               it->v_start, it->v_end, it->dgd_stride, it->src_stride, m, h);
@@ -666,18 +654,18 @@ static void stats_body(void* vctx, int i) {
     memcpy(c->M + (size_t)i * 49, m, sizeof(int64_t) * w2);
     memcpy(c->H + (size_t)i * 2401, h, sizeof(int64_t) * w2 * w2);
 }
-void ref_compute_stats_batch_bd(const void* dgd, const void* src, const RefStatsItem* items, int n, int64_t* M, int64_t* H, int bd) {
+void ref_compute_stats_batch_bd(const void* dgd, const void* src, const SvtB200StatsItem* items, int n, int64_t* M, int64_t* H, int bd) {
     StatsCtx c = {dgd, src, items, M, H, bd};
     par_for(n, 1, stats_body, &c);
 }
-void ref_compute_stats_batch(const uint8_t* dgd, const uint8_t* src, const RefStatsItem* items, int n, int64_t* M, int64_t* H) {
+void ref_compute_stats_batch(const uint8_t* dgd, const uint8_t* src, const SvtB200StatsItem* items, int n, int64_t* M, int64_t* H) {
     ref_compute_stats_batch_bd(dgd, src, items, n, M, H, 8);
 }
 
-typedef struct { const void* src; void* dst; const RefWienerUnit* units; int bd; } WienerCtx;
+typedef struct { const void* src; void* dst; const SvtB200WienerUnit* units; int bd; } WienerCtx;
 static void wiener_body(void* vctx, int i) {
     const WienerCtx* c = (const WienerCtx*)vctx;
-    const RefWienerUnit* u = &c->units[i];
+    const SvtB200WienerUnit* u = &c->units[i];
     /* the reference derives the kernel base by masking the low address bits (convolve.c:48-56) */
     DECLARE_ALIGNED(256, int16_t, fx[128]);
     DECLARE_ALIGNED(256, int16_t, fy[128]);
@@ -691,11 +679,11 @@ static void wiener_body(void* vctx, int i) {
         svt_av1_highbd_wiener_convolve_add_src(CONVERT_TO_BYTEPTR((const uint16_t*)c->src + u->src_off), u->src_stride,
                                                CONVERT_TO_BYTEPTR((uint16_t*)c->dst + u->dst_off), u->dst_stride, fx, fy, u->w, u->h, &cp, c->bd);
 }
-void ref_wiener_units_bd(const void* src, void* dst, const RefWienerUnit* units, int n, int bd) {
+void ref_wiener_units_bd(const void* src, void* dst, const SvtB200WienerUnit* units, int n, int bd) {
     WienerCtx c = {src, dst, units, bd};
     par_for(n, 16, wiener_body, &c);
 }
-void ref_wiener_units_8bit(const uint8_t* src, uint8_t* dst, const RefWienerUnit* units, int n) { ref_wiener_units_bd(src, dst, units, n, 8); }
+void ref_wiener_units_8bit(const uint8_t* src, uint8_t* dst, const SvtB200WienerUnit* units, int n) { ref_wiener_units_bd(src, dst, units, n, 8); }
 
 /* ---- whole frames --------------------------------------------------------------------------------------
  * One RefFrameJob = every buffer and work list of one frame of hot-path work (bench.py / FrameWorkload).
@@ -703,17 +691,16 @@ void ref_wiener_units_8bit(const uint8_t* src, uint8_t* dst, const RefWienerUnit
  * from the main thread); ref_frames_run keeps WHOLE FRAMES IN FLIGHT instead, one frame per pool thread, each
  * worker running its frame's calls serially into its own private output buffers -- how the encoder uses the
  * host cores (picture-level parallelism, enc_handle.c:770-781). */
-typedef struct { int32_t restoration_type, sgr_ep, sgr_xqd[2]; int16_t hfilter[8], vfilter[8]; } RefLrUnitInfo;
 void ref_lr_save_boundaries(void* plane_px00, int stride, int w, int h, int bit_depth, int plane, int frame_w, int frame_h, int after_cdef,
                             void* above, void* below, int bstride);
 void ref_lr_filter_plane(void* data, int stride, void* dst, int dst_stride, int w, int h, int ss_x, int ss_y, int bit_depth, int unit_size,
-                         const RefLrUnitInfo* units, void* above, void* below, int bstride, int optimized_lr);
+                         const SvtB200LrUnitInfo* units, void* above, void* below, int bstride, int optimized_lr);
 typedef struct RefFrameJob {
     int32_t width, height, bit_depth, n_refs;
-    const RefMePicture* cur; const RefMePicture* refs; const RefMeB64Cfg* me_cfg;
+    const SvtB200MePicture* cur; const SvtB200MePicture* refs; const RefMeB64Cfg* me_cfg;
     RefMeB64Out me; /* MeSbResults + distortions + per-reference state of svt_aom_motion_estimation_b64 (best_sad / best_mv unused: NULL) */
     int16_t* residual; int32_t *coeff, *q, *dq; const int16_t *scan, *iscan; const uint8_t* qm;
-    const RefFwdItem* fwd; const RefQuantItem* qi; const RefInvItem* inv; uint16_t* eobs;
+    const SvtB200FwdTxfmItem* fwd; const SvtB200QuantItem* qi; const SvtB200InvTxfmItem* inv; uint16_t* eobs;
     int64_t n_tx, n_coeffs;
     const void* pred; void* recon; void* cdef_out; void* final; const void* src;
     int64_t padded_elems;          /* pixels of one padded Y|U|V buffer */
@@ -723,11 +710,11 @@ typedef struct RefFrameJob {
     const uint8_t* skip; const int32_t *str_y, *str_uv; int32_t n_str, damping, subsampling, reserved1;
     uint64_t* mse; uint8_t* dir; int32_t* var;
     const int8_t* fb_idx; const int32_t *apply_y, *apply_uv;
-    const RefStatsItem* stats; int64_t *M, *H; const RefWienerUnit* units; int32_t n_stats, n_units;
-    const RefLrUnitInfo* lr_units[3]; void* lr_above[3]; void* lr_below[3]; int32_t lr_unit_size[3], lr_bstride[3], lr_stripes[3], reserved2;
+    const SvtB200StatsItem* stats; int64_t *M, *H; const SvtB200WienerUnit* units; int32_t n_stats, n_units;
+    const SvtB200LrUnitInfo* lr_units[3]; void* lr_above[3]; void* lr_below[3]; int32_t lr_unit_size[3], lr_bstride[3], lr_stripes[3], reserved2;
 } RefFrameJob;
 
-static void job_cdef_frame(const RefFrameJob* j, RefCdefFrame* f) {
+static void job_cdef_frame(const RefFrameJob* j, SvtB200CdefFrame* f) {
     const int psz = j->bit_depth > 8 ? 2 : 1;
     const void** rec[3] = {&f->recon_y, &f->recon_cb, &f->recon_cr};
     const void** src[3] = {&f->src_y, &f->src_cb, &f->src_cr};
@@ -778,7 +765,7 @@ void ref_frame_step(const RefFrameJob* j) {
     TRACE("me");
     const int nb = ((j->width + 63) >> 6) * ((j->height + 63) >> 6), psz = j->bit_depth > 8 ? 2 : 1;
     {   /* the reference's own open-loop ME driver for every 64x64 block (oracle/ref_me_b64.c) */
-        RefMeControls ctrl;
+        SvtB200MeControls ctrl;
         RefMeB64Out   mo = j->me;
         ref_me_b64_picture(j->cur, j->refs, j->me_cfg, &ctrl, &mo);
     }
@@ -791,7 +778,7 @@ void ref_frame_step(const RefFrameJob* j) {
     for (int p = 0; p < 3; p++)
         ref_lr_save_boundaries((uint8_t*)j->recon + (size_t)(j->plane_off[p] + (int64_t)j->pad * j->plane_stride[p] + j->pad) * psz, j->plane_stride[p],
                                j->plane_w[p], j->plane_h[p], j->bit_depth, p, j->width, j->height, 0, j->lr_above[p], j->lr_below[p], j->lr_bstride[p]);
-    RefCdefFrame f;
+    SvtB200CdefFrame f;
     job_cdef_frame(j, &f);
     CdefSearchCtx cs = {&f, j->skip, j->str_y, j->str_uv, j->n_str, j->mse, j->dir, j->var};
     par_for(nb, 2, cdef_search_body, &cs);
@@ -959,7 +946,7 @@ void ref_lr_save_boundaries(void* plane_px00, int stride, int w, int h, int bit_
 
 /* data: pixel (0,0) of a plane with >= 3 pixels of writable border (the reference extends it in place, :1223) */
 void ref_lr_filter_plane(void* data, int stride, void* dst, int dst_stride, int w, int h, int ss_x, int ss_y, int bit_depth, int unit_size,
-                         const RefLrUnitInfo* units, void* above, void* below, int bstride, int optimized_lr) {
+                         const SvtB200LrUnitInfo* units, void* above, void* below, int bstride, int optimized_lr) {
     const int highbd = bit_depth > 8;
     uint8_t* data8 = highbd ? CONVERT_TO_BYTEPTR((uint16_t*)data) : (uint8_t*)data;
     uint8_t* dst8 = highbd ? CONVERT_TO_BYTEPTR((uint16_t*)dst) : (uint8_t*)dst;
@@ -986,7 +973,7 @@ void ref_lr_filter_plane(void* data, int stride, void* dst, int dst_stride, int 
         while (x0 < w) {
             const int rem_w = w - x0, uw = rem_w < ext ? rem_w : unit_size;
             lim.h_start = x0; lim.h_end = x0 + uw;
-            const RefLrUnitInfo* u = &units[i * hunits + j];
+            const SvtB200LrUnitInfo* u = &units[i * hunits + j];
             RestorationUnitInfo  rui;
             memset(&rui, 0, sizeof(rui));
             rui.restoration_type = (RestorationType)u->restoration_type;

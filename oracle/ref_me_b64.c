@@ -27,7 +27,7 @@ extern void svt_aom_get_max_allocated_me_refs(uint8_t ref_count_used_list0, uint
 typedef void (*ParBody)(void* ctx, int i);
 extern void ref_par_for(int n, int chunk, ParBody body, void* ctx); /* ref_driver.c's pool */
 
-static void fill_desc(EbPictureBufferDesc* d, const RefMePicture* p, int level) {
+static void fill_desc(EbPictureBufferDesc* d, const SvtB200MePicture* p, int level) {
     memset(d, 0, sizeof(*d));
     d->buffer_y = (uint8_t*)p->plane[level];
     d->stride_y = (uint16_t)p->stride[level];
@@ -112,13 +112,8 @@ static void me_b64_row(void* vctx, int by) {
 }
 
 /* the flattened controls come from the integration glue a maintainer would ship (integration/svt_b200_me_glue.c): the parity
- * tests thereby check that mapping too.  RefMeControls and SvtB200MeControls are the same layout (static assert below). */
-#include "../include/svt_b200.h"
+ * tests thereby check that mapping too. */
 #include "../integration/svt_b200_me_glue.h"
-_Static_assert(sizeof(RefMeControls) == sizeof(SvtB200MeControls), "control struct mirrors differ");
-static void flatten_controls(const MeB64Job* j, const MeContext* me, RefMeControls* c) {
-    svt_b200_me_controls_from_context(j->pcs, me, (SvtB200MeControls*)c);
-}
 
 /* number of square PUs that carry candidates (me_sb_results_ctor, pcs.c:107-112) */
 int ref_me_b64_num_pus(int enc_mode, int width, int height) {
@@ -140,7 +135,8 @@ int ref_me_b64_sizes(const RefMeB64Cfg* cfg, int width, int height, int* n_pu, i
 
 /* refs: [n_ref[0] + n_ref[1]] descriptors, list 0 first.  Returns 0; fills *ctrl with the derived controls; when `out` is NULL only
  * derives the controls. */
-int ref_me_b64_picture(const RefMePicture* cur, const RefMePicture* refs, const RefMeB64Cfg* cfg, RefMeControls* ctrl, RefMeB64Out* out) {
+int ref_me_b64_picture(const SvtB200MePicture* cur, const SvtB200MePicture* refs, const RefMeB64Cfg* cfg, SvtB200MeControls* ctrl,
+                       RefMeB64Out* out) {
     MeB64Job j;
     memset(&j, 0, sizeof(j));
     const int W = cur->width[2], H = cur->height[2];
@@ -209,7 +205,7 @@ int ref_me_b64_picture(const RefMePicture* cur, const RefMePicture* refs, const 
     {
         MeContext* me = (MeContext*)calloc(1, sizeof(MeContext));
         setup_me_ctx(&j, me);
-        flatten_controls(&j, me, ctrl);
+        svt_b200_me_controls_from_context(pcs, me, ctrl);
         free(me->p_eight_pos_sad16x16);
         free(me);
     }

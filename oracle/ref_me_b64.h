@@ -1,10 +1,9 @@
-/* oracle/ref_me_b64.h -- TEST / BASELINE INFRASTRUCTURE: the structs of oracle/ref_me_b64.c (ctypes mirrors in oracle/support.py) */
+/* oracle/ref_me_b64.h -- TEST / BASELINE INFRASTRUCTURE: the entry points of oracle/ref_me_b64.c and the structs they take beyond
+ * include/svt_b200.h's (ctypes mirrors in oracle/support.py) */
 #ifndef REF_ME_B64_H
 #define REF_ME_B64_H
 #include <stdint.h>
-
-/* level 0 = 1/16, 1 = 1/4, 2 = full resolution luma */
-typedef struct { const uint8_t* plane[3]; int32_t stride[3], org_x[3], org_y[3], width[3], height[3], reserved[2]; } RefMePicture;
+#include "../include/svt_b200.h"
 
 /* what the caller chooses (the encoder derives these in resource coordination / picture decision) */
 typedef struct {
@@ -18,25 +17,6 @@ typedef struct {
     int32_t frame_rate_q16;           /* scs->frame_rate (Q16) */
     int32_t reserved[3];
 } RefMeB64Cfg;
-
-/* the derived MeContext controls, flattened: the layout of SvtB200MeControls (include/svt_b200.h) */
-typedef struct {
-    int32_t n_list, n_ref[2], temporal_layer_index, is_ref, hierarchical_levels;
-    int32_t dist[2][4];
-    int32_t enable_hme, enable_l0, enable_l1, enable_l2, hme_sub_sad, me_sub_sad;
-    int32_t hme_l0_min_w, hme_l0_min_h, hme_l0_max_w, hme_l0_max_h, hme_l1_w, hme_l1_h, hme_l2_w, hme_l2_h;
-    int32_t me_min_w, me_min_h, me_max_w, me_max_h;
-    int32_t prehme_enable, prehme_sa[2][4], prehme_skip_search_line, prehme_l1_early_exit;
-    int32_t prune_enable, prune_hme_th, prune_me_th, zz_sad_th, zz_sad_pct, phme_sad_th, phme_sad_pct;
-    int32_t sr_enable, sr_mv_length_th, sr_stationary_hme_sad_abs_th, sr_stationary_divisor, sr_hme_sad_abs_th, sr_low_hme_sad_divisor, sr_distance_based_hme_resizing;
-    int32_t var_enable, var_div4_th, var_div2_th, var_mult2_th;
-    int32_t mvsa_enable, mvsa_nearest_ref_only, mvsa_mv_size_th, mvsa_multiplier;
-    int32_t reduce_hme_l0_sr_th_min, reduce_hme_l0_sr_th_max;
-    int32_t me_early_exit_th, me_safe_limit_zz_th, prev_me_stage_based_exit_th, prune_me_candidates_th, use_best_unipred_cand_only;
-    int32_t similar_brightness_refs, only_l_bwd, enable_me_8x8, enable_me_16x16, max_cand, max_refs, max_l0;
-    int32_t gm_enabled, gm_use_distance_based_active_th, resolution_le_480p;
-    int32_t reserved[5];
-} RefMeControls;
 
 typedef struct {
     uint8_t*  total_me_candidate_index; /* [n_b64][n_pu] */
@@ -54,5 +34,6 @@ typedef struct {
 
 int ref_me_b64_num_pus(int enc_mode, int width, int height);
 int ref_me_b64_sizes(const RefMeB64Cfg* cfg, int width, int height, int* n_pu, int* max_cand, int* max_refs);
-int ref_me_b64_picture(const RefMePicture* cur, const RefMePicture* refs, const RefMeB64Cfg* cfg, RefMeControls* ctrl, RefMeB64Out* out);
+int ref_me_b64_picture(const SvtB200MePicture* cur, const SvtB200MePicture* refs, const RefMeB64Cfg* cfg, SvtB200MeControls* ctrl,
+                       RefMeB64Out* out);
 #endif

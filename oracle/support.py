@@ -1,25 +1,29 @@
-"""TEST / BASELINE INFRASTRUCTURE: ctypes mirrors of the structs taken by oracle/ref_driver.c and the
-numpy input preparation (padded HME pyramid) shared by tests/ and bench.py's reference arm."""
+"""TEST / BASELINE INFRASTRUCTURE: the structs oracle/ref_driver.c and oracle/ref_me_b64.c take beyond the product's
+(include/svt_b200.h, described by svt-av1-psy_b200/layout.py) and the numpy input preparation (padded HME pyramid) shared by
+tests/ and bench.py's reference arm."""
 import ctypes as ct
+import importlib
+import os
+import sys
 
 import numpy as np
 
-
-class RefMePicture(ct.Structure):
-    _fields_ = [("plane", ct.c_void_p * 3), ("stride", ct.c_int32 * 3), ("org_x", ct.c_int32 * 3), ("org_y", ct.c_int32 * 3),
-                ("width", ct.c_int32 * 3), ("height", ct.c_int32 * 3), ("reserved", ct.c_int32 * 2)]
+_PKG = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "svt-av1-psy_b200")
 
 
-class RefMeParams(ct.Structure):
-    _fields_ = [(n, ct.c_int32) for n in ("hme_l0_sa_w", "hme_l0_sa_h", "hme_l1_sa_w", "hme_l1_sa_h", "hme_l2_sa_w", "hme_l2_sa_h", "me_sa_w",
-                                          "me_sa_h", "hme_sub_sad", "me_sub_sad", "check_zero_centre", "reserved")]
+def load_pkg_module(name):
+    """svt-av1-psy_b200/<name>.py for the pure-numpy modules (layout, workload): the product package's own module when the
+    package is already imported (tests, H100 arm), else the file as a top-level module (no package __init__, no .so)"""
+    if "svt_av1_psy_b200." + name in sys.modules:
+        return sys.modules["svt_av1_psy_b200." + name]
+    if _PKG not in sys.path:
+        sys.path.append(_PKG)
+    return importlib.import_module(name)
 
 
-class RefCdefFrame(ct.Structure):
-    _fields_ = [("recon_y", ct.c_void_p), ("recon_cb", ct.c_void_p), ("recon_cr", ct.c_void_p), ("src_y", ct.c_void_p),
-                ("src_cb", ct.c_void_p), ("src_cr", ct.c_void_p), ("recon_stride_y", ct.c_int32), ("recon_stride_c", ct.c_int32),
-                ("src_stride_y", ct.c_int32), ("src_stride_c", ct.c_int32), ("width", ct.c_int32), ("height", ct.c_int32),
-                ("bit_depth", ct.c_int32), ("damping", ct.c_int32), ("subsampling_factor", ct.c_int32), ("reserved", ct.c_int32)]
+layout = load_pkg_module("layout")
+ME_CONTROL_FIELDS, MeControls, MePicture, MeParams, CdefFrame = \
+    layout.ME_CONTROL_FIELDS, layout.MeControls, layout.MePicture, layout.MeParams, layout.CdefFrame
 
 
 def pad_np(buf, pad, w, h):
@@ -48,7 +52,7 @@ def build_pyramid_np(full, width, height, shapes):
 
 
 def ref_pic_desc(planes, shapes):
-    p = RefMePicture()
+    p = MePicture()
     for lvl, (th, stride, pad, w, h) in enumerate(shapes):
         p.plane[lvl] = planes[lvl].ctypes.data
         p.stride[lvl] = stride
@@ -65,31 +69,6 @@ class RefMeB64Cfg(ct.Structure):
                [(n, ct.c_int32) for n in ("enable_hme_flag", "enable_hme_level0_flag", "enable_hme_level1_flag", "enable_hme_level2_flag",
                                           "max_l0", "max_l1", "only_l_bwd", "safe_limit_nref", "safe_limit_zz_th", "similar_brightness_refs",
                                           "gm_enabled", "gm_use_distance_based_active_th", "frame_rate_q16")] + [("reserved", ct.c_int32 * 3)]
-
-
-# field order == SvtB200MeControls (include/svt_b200.h) == RefMeControls (oracle/ref_me_b64.c)
-ME_CONTROL_FIELDS = [("n_list", 1), ("n_ref", 2), ("temporal_layer_index", 1), ("is_ref", 1), ("hierarchical_levels", 1), ("dist", 8),
-                     ("enable_hme", 1), ("enable_l0", 1), ("enable_l1", 1), ("enable_l2", 1), ("hme_sub_sad", 1), ("me_sub_sad", 1),
-                     ("hme_l0_min_w", 1), ("hme_l0_min_h", 1), ("hme_l0_max_w", 1), ("hme_l0_max_h", 1), ("hme_l1_w", 1), ("hme_l1_h", 1),
-                     ("hme_l2_w", 1), ("hme_l2_h", 1), ("me_min_w", 1), ("me_min_h", 1), ("me_max_w", 1), ("me_max_h", 1),
-                     ("prehme_enable", 1), ("prehme_sa", 8), ("prehme_skip_search_line", 1), ("prehme_l1_early_exit", 1),
-                     ("prune_enable", 1), ("prune_hme_th", 1), ("prune_me_th", 1), ("zz_sad_th", 1), ("zz_sad_pct", 1), ("phme_sad_th", 1),
-                     ("phme_sad_pct", 1), ("sr_enable", 1), ("sr_mv_length_th", 1), ("sr_stationary_hme_sad_abs_th", 1),
-                     ("sr_stationary_divisor", 1), ("sr_hme_sad_abs_th", 1), ("sr_low_hme_sad_divisor", 1), ("sr_distance_based_hme_resizing", 1),
-                     ("var_enable", 1), ("var_div4_th", 1), ("var_div2_th", 1), ("var_mult2_th", 1),
-                     ("mvsa_enable", 1), ("mvsa_nearest_ref_only", 1), ("mvsa_mv_size_th", 1), ("mvsa_multiplier", 1),
-                     ("reduce_hme_l0_sr_th_min", 1), ("reduce_hme_l0_sr_th_max", 1),
-                     ("me_early_exit_th", 1), ("me_safe_limit_zz_th", 1), ("prev_me_stage_based_exit_th", 1), ("prune_me_candidates_th", 1),
-                     ("use_best_unipred_cand_only", 1), ("similar_brightness_refs", 1), ("only_l_bwd", 1), ("enable_me_8x8", 1),
-                     ("enable_me_16x16", 1), ("max_cand", 1), ("max_refs", 1), ("max_l0", 1), ("gm_enabled", 1),
-                     ("gm_use_distance_based_active_th", 1), ("resolution_le_480p", 1), ("reserved", 5)]
-
-
-class RefMeControls(ct.Structure):
-    _fields_ = [(n, ct.c_int32 if k == 1 else ct.c_int32 * k) for n, k in ME_CONTROL_FIELDS]
-
-    def as_dict(self):
-        return {n: (int(getattr(self, n)) if k == 1 else [int(v) for v in getattr(self, n)]) for n, k in ME_CONTROL_FIELDS if n != "reserved"}
 
 
 class RefMeB64Out(ct.Structure):
@@ -121,8 +100,8 @@ def ref_me_b64_picture(ref, cur_pyr, ref_pyrs, shapes, cfg, run=True):
     ref.ref_me_b64_num_pus.restype = ct.c_int
     n_pu = ref.ref_me_b64_num_pus(cfg.enc_mode, W, H)
     cd = ref_pic_desc(cur_pyr, shapes)
-    rd = (RefMePicture * len(ref_pyrs))(*[ref_pic_desc(p, shapes) for p in ref_pyrs])
-    ctrl = RefMeControls()
+    rd = (MePicture * len(ref_pyrs))(*[ref_pic_desc(p, shapes) for p in ref_pyrs])
+    ctrl = MeControls()
     ref.ref_me_b64_picture.restype = ct.c_int
     ref.ref_me_b64_picture.argtypes = [ct.c_void_p] * 5
     if not run:

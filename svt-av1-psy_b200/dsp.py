@@ -9,7 +9,7 @@ import ctypes as ct
 import numpy as np
 
 from . import lib
-from .layout import *  # noqa: F401,F403  (struct dtypes, enum values and plane geometry: pure numpy, shared with the CPU arm)
+from .layout import *  # noqa: F401,F403  (the header's structs and item dtypes, enum values, plane geometry: no library, shared with the CPU arm)
 
 c_u8p = ct.POINTER(ct.c_uint8)
 c_u16p = ct.POINTER(ct.c_uint16)
@@ -28,15 +28,6 @@ def _ptr(a, typ=vp, byte_off=0):
         return ct.cast(0, typ)
     return ct.cast(a.ctypes.data + int(byte_off), typ)
 
-
-class SadSearchItem(ct.Structure):
-    _fields_ = [("src_off", ct.c_uint64), ("ref_off", ct.c_uint64), ("src_stride", ct.c_uint32),
-                ("ref_stride", ct.c_uint32), ("ref_step", ct.c_uint32), ("block_w", ct.c_uint16),
-                ("block_h", ct.c_uint16), ("sa_w", ct.c_int16), ("sa_h", ct.c_int16),
-                ("skip_search_line", ct.c_uint16), ("reserved", ct.c_uint16)]
-
-
-assert SAD_ITEM_DTYPE.itemsize == ct.sizeof(SadSearchItem) == 40
 
 # ------------------------------------------------------------------------------------------------
 # signatures
@@ -212,17 +203,6 @@ for _n, _extra in (("aom_quantize_b", [vp, vp, ct.c_int32]), ("aom_highbd_quanti
     _f.restype = None
 lib.svt_b200_residual_txfm_trio_batch_dev.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, ct.POINTER(ct.c_int), vp, ct.c_int, vp]
 lib.svt_b200_residual_txfm_trio_batch_dev.restype = ct.c_int
-
-
-class ResidualPlane(ct.Structure):  # SvtB200ResidualPlane
-    _fields_ = [("src_off", ct.c_uint64), ("pred_off", ct.c_uint64), ("res_off", ct.c_uint64), ("src_stride", ct.c_int32),
-                ("pred_stride", ct.c_int32), ("res_stride", ct.c_int32), ("w", ct.c_int32), ("h", ct.c_int32), ("reserved", ct.c_int32)]
-
-
-class ResidualPlanes(ct.Structure):
-    _fields_ = [("p", ResidualPlane * 3)]
-
-
 lib.svt_b200_residual_planes_dev.argtypes = [vp, vp, vp, ct.POINTER(ResidualPlanes), ct.c_int, ct.c_int, vp]
 lib.svt_b200_residual_planes_dev.restype = ct.c_int
 lib.svt_b200_pack_levels_dev.argtypes = [vp, vp, vp, vp, ct.c_int, vp, vp, ct.c_int, ct.c_uint32, vp]
@@ -260,10 +240,6 @@ for _n in ("4x4", "8x8", "16x16", "32x32"):
     _f.restype = None
 lib.svt_b200_aom_satd.argtypes = [vp, ct.c_int]
 lib.svt_b200_aom_satd.restype = ct.c_int
-class Buf2D(ct.Structure):  # SvtB200Buf2D == the reference's Buf2D
-    _fields_ = [("buf", vp), ("buf0", vp), ("width", ct.c_int), ("height", ct.c_int), ("stride", ct.c_int)]
-
-
 lib.svt_b200_hadamard_path.argtypes = [Buf2D, Buf2D, Buf2D, Buf2D, ct.c_uint8]
 lib.svt_b200_hadamard_path.restype = ct.c_uint32
 lib.svt_b200_av1_fwht4x4.argtypes = [vp, vp, ct.c_uint32]
@@ -313,13 +289,6 @@ def fullpel_search_batch_host(src_plane, ref_plane, items):
 # ------------------------------------------------------------------------------------------------
 # K8 CDEF
 # ------------------------------------------------------------------------------------------------
-class CdefFrame(ct.Structure):
-    _fields_ = [("recon_y", vp), ("recon_cb", vp), ("recon_cr", vp), ("src_y", vp), ("src_cb", vp), ("src_cr", vp),
-                ("recon_stride_y", ct.c_int32), ("recon_stride_c", ct.c_int32), ("src_stride_y", ct.c_int32),
-                ("src_stride_c", ct.c_int32), ("width", ct.c_int32), ("height", ct.c_int32), ("bit_depth", ct.c_int32),
-                ("damping", ct.c_int32), ("subsampling_factor", ct.c_int32), ("reserved", ct.c_int32)]
-
-
 lib.svt_b200_aom_cdef_find_dir.argtypes = [vp, ct.c_int32, vp, ct.c_int32]
 lib.svt_b200_aom_cdef_find_dir.restype = ct.c_uint8
 lib.svt_b200_aom_cdef_find_dir_dual.argtypes = [vp, vp, ct.c_int, vp, vp, ct.c_int32, vp, vp]
@@ -354,13 +323,6 @@ def cdef_frame_desc(rec, src, width, height, bit_depth, damping, subsampling):
 # ------------------------------------------------------------------------------------------------
 # K9 / K11 Wiener
 # ------------------------------------------------------------------------------------------------
-class ConvolveParams(ct.Structure):
-    _fields_ = [("ref", ct.c_int32), ("do_average", ct.c_int32), ("dst", vp), ("dst_stride", ct.c_int32),
-                ("round_0", ct.c_int32), ("round_1", ct.c_int32), ("plane", ct.c_int32), ("is_compound", ct.c_int32),
-                ("use_jnt_comp_avg", ct.c_int32), ("fwd_offset", ct.c_int32), ("bck_offset", ct.c_int32),
-                ("use_dist_wtd_comp_avg", ct.c_int32)]
-
-
 lib.svt_b200_av1_wiener_convolve_add_src.argtypes = [vp, ct.c_ssize_t, vp, ct.c_ssize_t, vp, vp, ct.c_int32, ct.c_int32,
                                                      ct.POINTER(ConvolveParams)]
 lib.svt_b200_av1_wiener_convolve_add_src.restype = None
@@ -397,13 +359,6 @@ lib.svt_b200_sgr_units_dev.restype = ct.c_int
 # ------------------------------------------------------------------------------------------------
 # a13 loop-restoration drivers
 # ------------------------------------------------------------------------------------------------
-class LrPlane(ct.Structure):  # SvtB200LrPlane
-    _fields_ = [("deblocked", vp), ("cdef", vp), ("dst", vp), ("src", vp), ("boundary_above", vp), ("boundary_below", vp),
-                ("stride_deblocked", ct.c_int32), ("stride_cdef", ct.c_int32), ("stride_dst", ct.c_int32), ("stride_src", ct.c_int32),
-                ("boundary_stride", ct.c_int32), ("width", ct.c_int32), ("height", ct.c_int32), ("ss_x", ct.c_int32), ("ss_y", ct.c_int32),
-                ("unit_size", ct.c_int32), ("frame_restoration_type", ct.c_int32)]
-
-
 lib.svt_b200_lr_num_stripes.argtypes = [ct.c_int, ct.c_int]
 lib.svt_b200_lr_num_stripes.restype = ct.c_int
 lib.svt_b200_lr_boundary_stride.argtypes = [ct.c_int]
@@ -420,48 +375,12 @@ lib.svt_b200_lr_unit_sse_dev.restype = ct.c_int
 # ------------------------------------------------------------------------------------------------
 # K13 + T2 open-loop ME for a whole picture
 # ------------------------------------------------------------------------------------------------
-class MePicture(ct.Structure):
-    _fields_ = [("plane", vp * 3), ("stride", ct.c_int32 * 3), ("org_x", ct.c_int32 * 3), ("org_y", ct.c_int32 * 3),
-                ("width", ct.c_int32 * 3), ("height", ct.c_int32 * 3), ("reserved", ct.c_int32 * 2)]
-
-
-class MeParams(ct.Structure):
-    _fields_ = [("hme_l0_sa_w", ct.c_int32), ("hme_l0_sa_h", ct.c_int32), ("hme_l1_sa_w", ct.c_int32), ("hme_l1_sa_h", ct.c_int32),
-                ("hme_l2_sa_w", ct.c_int32), ("hme_l2_sa_h", ct.c_int32), ("me_sa_w", ct.c_int32), ("me_sa_h", ct.c_int32),
-                ("hme_sub_sad", ct.c_int32), ("me_sub_sad", ct.c_int32), ("check_zero_centre", ct.c_int32), ("reserved", ct.c_int32)]
-
-
 lib.svt_b200_downsample_2d.argtypes = [vp, ct.c_uint32, ct.c_uint32, ct.c_uint32, vp, ct.c_uint32, ct.c_uint32]
 lib.svt_b200_downsample_2d.restype = None
 lib.svt_b200_build_hme_pyramid_dev.argtypes = [ct.POINTER(MePicture), vp]
 lib.svt_b200_build_hme_pyramid_dev.restype = ct.c_int
 lib.svt_b200_me_picture_dev.argtypes = [ct.POINTER(MePicture), ct.POINTER(MePicture), ct.POINTER(MeParams), ct.c_int, vp, vp, vp, vp, vp]
 lib.svt_b200_me_picture_dev.restype = ct.c_int
-
-
-class MeControls(ct.Structure):  # SvtB200MeControls
-    _fields_ = [(n, ct.c_int32 if k == 1 else ct.c_int32 * k) for n, k in ME_CONTROL_FIELDS]
-
-    @classmethod
-    def from_dict(cls, d):
-        """d: field -> int (or a flat list for the array fields), e.g. the reference's derivation dumped by tools/dump_me_controls.py"""
-        c = cls()
-        for n, k in ME_CONTROL_FIELDS:
-            if n == "reserved" or n not in d:
-                continue
-            if k == 1:
-                setattr(c, n, int(d[n]))
-            else:
-                for i, v in enumerate(d[n]):
-                    getattr(c, n)[i] = int(v)
-        return c
-
-
-class MeB64Results(ct.Structure):  # SvtB200MeB64Results
-    _fields_ = [(n, vp) for n in ME_B64_RESULT_FIELDS]
-
-
-assert ct.sizeof(MeControls) == 4 * ME_CONTROL_WORDS
 lib.svt_b200_me_b64_num_pus.argtypes = [ct.POINTER(MeControls)]
 lib.svt_b200_me_b64_num_pus.restype = ct.c_int
 lib.svt_b200_me_b64_picture_dev.argtypes = [ct.POINTER(MePicture), ct.POINTER(MePicture), ct.POINTER(MeControls), ct.POINTER(MeB64Results), vp]
@@ -482,13 +401,6 @@ def me_picture_desc(planes, width, height):
     return p
 lib.svt_b200_extend_plane_dev.argtypes = [vp, ct.c_int, ct.c_int, ct.c_int, ct.c_int, ct.c_int, vp]
 lib.svt_b200_extend_plane_dev.restype = ct.c_int
-
-
-class PlaneExtent(ct.Structure):  # SvtB200PlaneExtent
-    _fields_ = [("buf", ct.c_void_p), ("stride", ct.c_int32), ("w", ct.c_int32), ("h", ct.c_int32), ("org_x", ct.c_int32),
-                ("org_y", ct.c_int32), ("pixel_bytes", ct.c_int32)]
-
-
 lib.svt_b200_extend_planes_dev.argtypes = [ct.POINTER(PlaneExtent), ct.c_int, vp]
 lib.svt_b200_extend_planes_dev.restype = ct.c_int
 

@@ -6,6 +6,8 @@ import ctypes as ct
 
 import numpy as np
 
+from oracle import support as sp
+
 BS, VL = 144, 0x7f7f
 
 
@@ -145,18 +147,12 @@ def ref_cdef_apply(refc, rec, skip, width, height, bd, damping, fb_idx, str_y, s
     return filtered, dirs, vars_
 
 
-class RefCdefFrame(ct.Structure):  # RefCdefFrame (oracle/ref_driver.c) == SvtB200CdefFrame
-    _fields_ = [(n, ct.c_void_p) for n in ("recon_y", "recon_cb", "recon_cr", "src_y", "src_cb", "src_cr")] + \
-               [(n, ct.c_int32) for n in ("recon_stride_y", "recon_stride_c", "src_stride_y", "src_stride_c", "width", "height",
-                                          "bit_depth", "damping", "subsampling_factor", "reserved")]
-
-
 def _ref_frame(rec, src, width, height, bd, damping, subsampling):
-    """RefCdefFrame over copies of the planes in the pixel type of the bit depth, 8 padding pixels right of every row
+    """CdefFrame over copies of the planes in the pixel type of the bit depth, 8 padding pixels right of every row
     (fill_tile); the copies are returned to keep them alive"""
     dt = np.uint8 if bd == 8 else np.uint16
     keep = [np.pad(p.astype(dt), ((0, 0), (0, 8))) for p in list(rec) + list(src)]
-    f = RefCdefFrame()
+    f = sp.CdefFrame()
     f.recon_y, f.recon_cb, f.recon_cr, f.src_y, f.src_cb, f.src_cr = (k.ctypes.data for k in keep)
     f.recon_stride_y, f.recon_stride_c = keep[0].shape[1], keep[1].shape[1]
     f.src_stride_y, f.src_stride_c = keep[3].shape[1], keep[4].shape[1]

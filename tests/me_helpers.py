@@ -6,6 +6,8 @@ import ctypes as ct
 
 import numpy as np
 
+from oracle import support as sp
+
 MAX_SAD = 128 * 128 * 255
 
 
@@ -193,36 +195,15 @@ def ref_me_picture(refc, cur, refs, shapes, width, height, params, sad_fn="svt_s
     return out_sad, out_mv, out_c, out_hs
 
 
-class RefMePicture(ct.Structure):
-    _fields_ = [("plane", ct.c_void_p * 3), ("stride", ct.c_int32 * 3), ("org_x", ct.c_int32 * 3), ("org_y", ct.c_int32 * 3),
-                ("width", ct.c_int32 * 3), ("height", ct.c_int32 * 3), ("reserved", ct.c_int32 * 2)]
-
-
-class RefMeParams(ct.Structure):
-    _fields_ = [(n, ct.c_int32) for n in ("hme_l0_sa_w", "hme_l0_sa_h", "hme_l1_sa_w", "hme_l1_sa_h", "hme_l2_sa_w", "hme_l2_sa_h", "me_sa_w",
-                                          "me_sa_h", "hme_sub_sad", "me_sub_sad", "check_zero_centre", "reserved")]
-
-
-def ref_pic_desc(planes, shapes):
-    p = RefMePicture()
-    for lvl, (th, stride, pad, w, h) in enumerate(shapes):
-        p.plane[lvl] = planes[lvl].ctypes.data
-        p.stride[lvl] = stride
-        p.org_x[lvl] = p.org_y[lvl] = pad
-        p.width[lvl] = w
-        p.height[lvl] = h
-    return p
-
-
 def ref_me_picture_c(refc, cur, refs, shapes, width, height, params):
     """the pthread C driver in oracle/ref_driver.c (reference kernels through the dispatch pointers)"""
     R = len(refs)
     nb = ((width + 63) // 64) * ((height + 63) // 64)
     sad = np.zeros((R, nb, 85), np.uint32); mv = np.zeros((R, nb, 85), np.uint32)
     c = np.zeros((R, nb, 2), np.int16); hs = np.zeros((R, nb), np.uint64)
-    cd = ref_pic_desc(cur, shapes)
-    rd = (RefMePicture * R)(*[ref_pic_desc(r, shapes) for r in refs])
-    pr = (RefMeParams * R)()
+    cd = sp.ref_pic_desc(cur, shapes)
+    rd = (sp.MePicture * R)(*[sp.ref_pic_desc(r, shapes) for r in refs])
+    pr = (sp.MeParams * R)()
     for i, p in enumerate(params):
         for k, v in p.items():
             setattr(pr[i], k, v)

@@ -1,8 +1,9 @@
-"""CPU-only checks of the host side: the C structs of include/svt_b200.h against the numpy / ctypes mirrors,
+"""CPU-only checks of the host side: the C structs of include/svt_b200.h against their ctypes twins in layout.py,
 the batch-ordering rules of the transform calls, the synthetic workload's invariants, and the oracle pin of
 the N2 / N4 partial transforms (the fact the CUDA kernels rely on)."""
 import ctypes as ct
 import os
+import re
 import subprocess
 import tempfile
 
@@ -12,25 +13,46 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _c_sizes(names):
-    src = '#include <stdio.h>\n#include "svt_b200.h"\nint main(void){' + "".join(
-        'printf("%s %%zu\\n", sizeof(%s));' % (n, n) for n in names) + "return 0;}"
+def _c_layout(classes):
+    """{(struct, None): sizeof, (struct, field): (offsetof, sizeof member)} of the header, for the fields of each class"""
+    lines = []
+    for n, cls in classes.items():
+        lines.append('printf("%s - %%zu\\n", sizeof(SvtB200%s));' % (n, n))
+        lines += ['printf("%s %s %%zu %%zu\\n", offsetof(SvtB200%s, %s), sizeof(((SvtB200%s*)0)->%s));' % (n, f, n, f, n, f)
+                  for f, *_ in cls._fields_]
+    src = '#include <stddef.h>\n#include <stdio.h>\n#include "svt_b200.h"\nint main(void){\n' + "\n".join(lines) + "\nreturn 0;}\n"
     with tempfile.TemporaryDirectory() as d:
         c, exe = os.path.join(d, "s.c"), os.path.join(d, "s")
         open(c, "w").write(src)
-        subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), c, "-o", exe], check=True)
+        r = subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), c, "-o", exe], capture_output=True, text=True)
+        assert r.returncode == 0, r.stderr
         out = subprocess.run([exe], capture_output=True, text=True, check=True).stdout
-    return {l.split()[0]: int(l.split()[1]) for l in out.splitlines()}
+    got = {}
+    for l in out.splitlines():
+        n, f, *v = l.split()
+        got[n, None if f == "-" else f] = int(v[0]) if f == "-" else tuple(map(int, v))
+    return got
 
 
 def test_struct_layouts_match_the_header():
-    from svt_av1_psy_b200 import dsp
-    pairs = {"SvtB200FwdTxfmItem": dsp.FWD_ITEM_DTYPE.itemsize, "SvtB200InvTxfmItem": dsp.INV_ITEM_DTYPE.itemsize,
-             "SvtB200QuantItem": dsp.QUANT_ITEM_DTYPE.itemsize, "SvtB200TrioItem": dsp.TRIO_ITEM_DTYPE.itemsize,
-             "SvtB200StatsItem": dsp.STATS_ITEM_DTYPE.itemsize, "SvtB200WienerUnit": dsp.WIENER_UNIT_DTYPE.itemsize,
-             "SvtB200CdefFrame": ct.sizeof(dsp.CdefFrame), "SvtB200PlaneExtent": ct.sizeof(dsp.PlaneExtent)}
-    sizes = _c_sizes(list(pairs))
-    assert sizes == pairs
+    """Every `typedef struct SvtB200X` of the header has a twin layout.X and no class lacks one; every field of a twin has
+    the header's offset and size, and the fields tile the struct without gaps (only tail padding may stay unnamed)."""
+    import svt_av1_psy_b200
+    from svt_av1_psy_b200 import layout
+    txt = subprocess.run(["gcc", "-E", "-P", svt_av1_psy_b200.HEADER_PATH], capture_output=True, text=True, check=True).stdout
+    header = sorted(n[len("SvtB200"):] for n in set(re.findall(r"\btypedef\s+struct\s+(SvtB200\w+)", txt)))
+    classes = {n: c for n, c in vars(layout).items() if isinstance(c, type) and issubclass(c, ct.Structure)}
+    assert sorted(classes) == header
+    mine = {}
+    for n, cls in classes.items():
+        mine[n, None] = ct.sizeof(cls)
+        end = 0
+        for f, *_ in cls._fields_:
+            d = getattr(cls, f)
+            mine[n, f] = (d.offset, d.size)
+            assert d.offset == end, "%s: %d unnamed bytes before %s" % (n, d.offset - end, f)
+            end = d.offset + d.size
+    assert mine == _c_layout(classes)
 
 
 def test_team_class_rule_and_library_agree():
