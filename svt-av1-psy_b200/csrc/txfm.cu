@@ -176,6 +176,20 @@ inv_txfm_kernel(const int32_t* __restrict__ coef_base, const PIX* __restrict__ p
 // (the per-block chain of the final encode pass, coding_loop.c:405-658) without leaving shared memory:
 // the coefficients and the dequantised levels never travel through HBM between the three steps.
 // ------------------------------------------------------------------------------------------------
+// the 1-D passes of the fused kernel: in the big-block classes (one block per CTA of 2 * TEAM threads) 32- and 64-point
+// vectors run split across two lanes, shorter ones one per thread
+template <int TEAM, int THREADS, bool INV>
+__device__ __forceinline__ void trio_pass(int type, int32_t* x, int N, int V, int P, int cos_bit, int clampb, int tid) {
+    if constexpr (TEAM >= 32) {
+        static_assert(THREADS == 2 * TEAM, "a lane pair per vector");
+        if (N == 32) return txfm_pass_split<32, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
+        if constexpr (TEAM >= 64) {
+            if (N == 64) return txfm_pass_split<64, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
+        }
+    }
+    txfm_pass_1d<TEAM, INV, true>(type, x, N, V, P, cos_bit, clampb, tid);
+}
+
 template <int TEAM, int THREADS, typename PIX>
 __global__ void __launch_bounds__(THREADS)
 trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ srcpix_base /*non-null: residual = source - prediction, formed here*/,
@@ -184,8 +198,8 @@ trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ s
                  const uint8_t* __restrict__ qm_base, const SvtB200TrioItem* __restrict__ items, int n_items,
                  uint16_t* __restrict__ eobs) {
     extern __shared__ __align__(16) int32_t tsm[];
-    // big blocks are few: one block per CTA (SOLO), all THREADS move its data, the first TEAM run the passes --
-    // the block's critical path is global-memory round trips, and 4x the movers means 4x fewer of them
+    // big blocks are few: one block per CTA (SOLO) of 2 * TEAM threads; all of them move its data, and lane pairs run
+    // its 32- and 64-point vectors (trio_pass)
     constexpr bool SOLO = TEAM >= 32;
     constexpr int  TEAMS = SOLO ? 1 : THREADS / TEAM, PLANE = TEAM * (TEAM + 1), MOVERS = SOLO ? THREADS : TEAM;
     const int      team  = SOLO ? 0 : threadIdx.x / TEAM, tid = SOLO ? threadIdx.x : threadIdx.x % TEAM;
@@ -223,7 +237,7 @@ trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ s
                 }
             }
             team_sync<TEAM, SOLO>();
-            txfm_pass_1d<TEAM, false, true>(cfg.f_tc, A, H, W, P1, cfg.f_cbc, 0, tid);  // rows >= Hp of the result are not needed
+            trio_pass<TEAM, THREADS, false>(cfg.f_tc, A, H, W, P1, cfg.f_cbc, 0, tid);  // rows >= Hp of the result are not needed
             team_sync<TEAM, SOLO>();
 #pragma unroll 4
             for (int idx = tid; idx < W * Hp; idx += MOVERS) {  // only the Hp rows that survive the packing
@@ -232,12 +246,12 @@ trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ s
                 B[cc * P2 + r] = round_shift_arr(A[r * P1 + c], -cfg.f_s1);
             }
             team_sync<TEAM, SOLO>();
-            txfm_pass_1d<TEAM, false, true>(cfg.f_tr, B, W, Hp, P2, cfg.f_cbr, 0, tid);
+            trio_pass<TEAM, THREADS, false>(cfg.f_tr, B, W, Hp, P2, cfg.f_cbr, 0, tid);
             team_sync<TEAM, SOLO>();
         }
         int block_eob = 0;
         {   // ---- quantise the (packed) coefficients; the dequantised levels become the inverse's input plane ----
-            const SvtB200QuantItem qi = item.quant;
+            const SvtB200QuantItem& qi = item.quant;
             const uint8_t* qm  = qi.qm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.qm_off;
             const uint8_t* iqm = qi.iqm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.iqm_off;
             const int16_t* iscan = iscan_base + qi.scan_off;
@@ -298,7 +312,7 @@ trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ s
             const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
             const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);
             const int opt_col = bd == 12 ? 18 : 16;
-            txfm_pass_1d<TEAM, true, true>(cfg.i_tr, A, W, Hp, P1, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
+            trio_pass<TEAM, THREADS, true>(cfg.i_tr, A, W, Hp, P1, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
             team_sync<TEAM, SOLO>();
 #pragma unroll 4
             for (int idx = tid; idx < W * H; idx += MOVERS) {
@@ -307,7 +321,7 @@ trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ s
                 B[r * P2 + c] = clamp_bits(round_shift_arr(A[cs * P1 + r], -cfg.i_s0), col_clamp);
             }
             team_sync<TEAM, SOLO>();
-            txfm_pass_1d<TEAM, true, true>(cfg.i_tc, B, H, W, P2, cfg.i_cbc, opt_col, tid);
+            trio_pass<TEAM, THREADS, true>(cfg.i_tc, B, H, W, P2, cfg.i_cbc, opt_col, tid);
             team_sync<TEAM, SOLO>();
             const PIX* pr = pred_base + item.inv.pred_off;
             PIX*       pw = recon_base + item.inv.recon_off;
@@ -391,7 +405,7 @@ template <int TEAM, typename PIX>
 static void launch_trio_class(const int16_t* d_src, const PIX* d_srcpix, const PIX* d_pred, PIX* d_recon, int32_t* d_q, int32_t* d_dq, const int16_t* d_iscan,
                               const uint8_t* d_qm, const SvtB200TrioItem* d_items, int n, uint16_t* d_eobs, cudaStream_t st) {
     if (n <= 0) return;
-    constexpr int    THREADS = TEAM == 32 ? 128 : class_threads<TEAM>(), TEAMS = TEAM >= 32 ? 1 : THREADS / TEAM;
+    constexpr int    THREADS = TEAM >= 32 ? 2 * TEAM : class_threads<TEAM>(), TEAMS = TEAM >= 32 ? 1 : THREADS / TEAM;
     constexpr size_t smem = (size_t)TEAMS * team_stride(TEAM) * 4;
     static int attr = -1;  // the initialisation (epoch) the attribute was applied in
     if (attr != epoch()) { set_smem_attr(trio_txfm_kernel<TEAM, THREADS, PIX>, smem); attr = epoch(); }

@@ -9,7 +9,8 @@
 // one thread holds one whole vector in registers -- stage permutations cost nothing and every
 // butterfly is a handful of integer instructions.  A team of max(W,H) threads owns a block: thread v
 // transforms column v, the block is handed over transposed through shared memory (odd pitch, so
-// both directions are bank-conflict free), then thread r transforms row r.
+// both directions are bank-conflict free), then thread r transforms row r.  In the fused kernel's 32- and 64-point
+// classes a 32- or 64-point DCT vector is split across two lanes instead (txfm_pass_split).
 #pragma once
 #include <cstdint>
 #include "common.cuh"
@@ -33,14 +34,19 @@ __constant__ TxCfg     c_txcfg[19][16];
 __constant__ int32_t   c_cospi[7][64];  // bit 10..16
 __constant__ int32_t   c_sinpi[7][5];
 
-__host__ __device__ constexpr int tx_w(int s) {
+// log2(dimension) - 2 of the 19 sizes, 3 bits each: a runtime-indexed constexpr array would be placed in local memory
+constexpr unsigned long long kTxLgW = 0x1132846d2244688ull;  // W: 4 8 16 32 64 4 8 8 16 16 32 32 64 4 16 8 32 16 64
+constexpr unsigned long long kTxLgH = 0x0a161389940c688ull;  // H: 4 8 16 32 64 8 4 16 8 32 16 64 32 16 4 32 8 64 16
+__host__ __device__ constexpr int tx_w(int s) { return 4 << ((kTxLgW >> (3 * s)) & 7); }
+__host__ __device__ constexpr int tx_h(int s) { return 4 << ((kTxLgH >> (3 * s)) & 7); }
+constexpr bool tx_dims_packed_right() {
     constexpr int W[19] = {4, 8, 16, 32, 64, 4, 8, 8, 16, 16, 32, 32, 64, 4, 16, 8, 32, 16, 64};
-    return W[s];
-}
-__host__ __device__ constexpr int tx_h(int s) {
     constexpr int H[19] = {4, 8, 16, 32, 64, 8, 4, 16, 8, 32, 16, 64, 32, 16, 4, 32, 8, 64, 16};
-    return H[s];
+    for (int s = 0; s < 19; s++)
+        if (tx_w(s) != W[s] || tx_h(s) != H[s]) return false;
+    return true;
 }
+static_assert(tx_dims_packed_right(), "kTxLgW / kTxLgH");
 const TxCfg& host_txcfg(int size, int type);
 
 constexpr int kNewSqrt2    = 5793;  // 2^12 * sqrt(2)
@@ -116,16 +122,17 @@ __device__ __forceinline__ void txfm_adst4(int32_t (&x)[4], int cos_bit) {
 
 // identity kernels (transforms.c:2205-2236, inv_transforms.c:2331-2362)
 template <int N>
+__device__ __forceinline__ int32_t txfm_identity_one(int32_t xv) {
+    if constexpr (N == 4) return round_shift64((long long)xv * kNewSqrt2, 12);
+    else if constexpr (N == 8) return (int32_t)((uint32_t)xv * 2u);
+    else if constexpr (N == 16) return round_shift64((long long)xv * 2 * kNewSqrt2, 12);
+    else if constexpr (N == 32) return (int32_t)((uint32_t)xv * 4u);
+    else return round_shift64((long long)xv * 4 * kNewSqrt2, 12);
+}
+template <int N>
 __device__ __forceinline__ void txfm_identity(int32_t (&x)[N]) {
 #pragma unroll
-    for (int i = 0; i < N; i++) {
-        const int32_t xv = x[i];
-        if constexpr (N == 4) x[i] = round_shift64((long long)xv * kNewSqrt2, 12);
-        else if constexpr (N == 8) x[i] = (int32_t)((uint32_t)xv * 2u);
-        else if constexpr (N == 16) x[i] = round_shift64((long long)xv * 2 * kNewSqrt2, 12);
-        else if constexpr (N == 32) x[i] = (int32_t)((uint32_t)xv * 4u);
-        else x[i] = round_shift64((long long)xv * 4 * kNewSqrt2, 12);
-    }
+    for (int i = 0; i < N; i++) x[i] = txfm_identity_one<N>(x[i]);
 }
 
 // one N-point vector in registers through the 1-D kernel `type` (a TT_* of that length)
@@ -181,6 +188,88 @@ __device__ __forceinline__ void txfm_pass_1d(int type, int32_t* x, int N, int V,
     if constexpr (TEAM >= 16) { if (N == 16) return txfm_pass_n<16, TEAM, INV, PACKED>(type, x, V, P, cos_bit, clampb, tid); }
     if constexpr (TEAM >= 32) { if (N == 32) return txfm_pass_n<32, TEAM, INV, PACKED>(type, x, V, P, cos_bit, clampb, tid); }
     if constexpr (TEAM >= 64) { if (N == 64) return txfm_pass_n<64, TEAM, INV, PACKED>(type, x, V, P, cos_bit, clampb, tid); }
+}
+
+// One 1-D pass of N = 32 or 64 points with every vector split across two lanes, for a block that has its CTA of
+// THREADS threads to itself: thread (g, v) = (tid / HALF, tid % HALF), HALF = THREADS / 2 >= V, runs lane group g
+// of vector v.  HALF >= 32, so g is warp-uniform and the two groups' different code never diverges within a warp.
+// DCT: the generated split (txfm_gen.inc, TxgSplit_*): forward, each group loads the vector and computes its own
+// outputs; inverse, each group computes its half of the values before the combining last stage, the halves meet
+// in shared memory, and each group runs the last stage for its outputs.  Identity: each group takes half the
+// elements.  Every thread of the CTA must call it (it holds the CTA's barriers).
+template <class S, int G, int N>
+__device__ __forceinline__ void split_mid(int32_t (&r)[N], int32_t* x, int P, int v, const int32_t* cosv, int cos_bit, int clampb) {
+    S::template mid<G>(r, cosv, cos_bit, clampb);
+    if constexpr (S::kTail) {
+        constexpr unsigned long long MID = G ? S::kMid1 : S::kMid0;
+#pragma unroll
+        for (int i = 0; i < N; i++)
+            if ((MID >> i) & 1) x[i * P + v] = r[i];
+    }
+}
+template <class S, int G, int N>
+__device__ __forceinline__ void split_tail(int32_t (&r)[N], int32_t* x, int P, int v, const int32_t* cosv, int cos_bit, int clampb) {
+    constexpr unsigned long long MID = G ? S::kMid1 : S::kMid0;
+#pragma unroll
+    for (int i = 0; i < N; i++)
+        if (!((MID >> i) & 1)) r[i] = x[i * P + v];  // the other group's values
+    S::template tail<G>(r, cosv, cos_bit, clampb);
+}
+template <class S, int G, int N>
+__device__ __forceinline__ void split_store(const int32_t (&r)[N], int32_t* x, int P, int v) {
+    constexpr unsigned long long OUT = G ? S::kOut1 : S::kOut0;
+#pragma unroll
+    for (int i = 0; i < N; i++)
+        if ((OUT >> i) & 1) x[i * P + v] = r[i];
+}
+template <class S, int N>
+__device__ __forceinline__ void txfm_pass_split_dct(int32_t* x, int V, int P, int cos_bit, int clampb, int g, int v) {
+    const int32_t* cosv = c_cospi[cos_bit - 10];
+    const bool on = v < V;
+    int32_t r[N];
+    if (on) {
+#pragma unroll
+        for (int i = 0; i < N; i++) r[i] = x[i * P + v];  // loads outside the group's network are dead
+    }
+    __syncthreads();  // both groups have read the vector before either writes over it
+    if (on) {
+        if (g == 0) split_mid<S, 0>(r, x, P, v, cosv, cos_bit, clampb);
+        else split_mid<S, 1>(r, x, P, v, cosv, cos_bit, clampb);
+    }
+    if constexpr (S::kTail) {
+        __syncthreads();  // both halves are in shared memory
+        if (on) {
+            if (g == 0) split_tail<S, 0>(r, x, P, v, cosv, cos_bit, clampb);
+            else split_tail<S, 1>(r, x, P, v, cosv, cos_bit, clampb);
+        }
+        __syncthreads();  // both groups have read the other's half before the outputs go over it
+    }
+    if (on) {
+        if (g == 0) split_store<S, 0>(r, x, P, v);
+        else split_store<S, 1>(r, x, P, v);
+    }
+}
+template <int N, int THREADS, bool INV>
+__device__ __forceinline__ void txfm_pass_split(int type, int32_t* x, int V, int P, int cos_bit, int clampb, int tid) {
+    static_assert(N == 32 || N == 64, "two-lane splits exist for 32 and 64 points");
+    constexpr int HALF = THREADS / 2;
+    static_assert(HALF >= 32 && HALF % 32 == 0, "lane groups are whole warps");
+    const int g = tid / HALF, v = tid % HALF;
+    if (type == (N == 32 ? TT_DCT32 : TT_DCT64)) {
+        if constexpr (N == 32 && INV) txfm_pass_split_dct<TxgSplit_IDCT32, 32>(x, V, P, cos_bit, clampb, g, v);
+        else if constexpr (N == 32) txfm_pass_split_dct<TxgSplit_FDCT32, 32>(x, V, P, cos_bit, clampb, g, v);
+        else if constexpr (INV) txfm_pass_split_dct<TxgSplit_IDCT64_in32, 64>(x, V, P, cos_bit, clampb, g, v);
+        else txfm_pass_split_dct<TxgSplit_FDCT64_lo32, 64>(x, V, P, cos_bit, clampb, g, v);
+    } else if (v < V) {
+        // identity, element-wise.  64 points are packed: the forward's elements 32..63 are not kept, the inverse's
+        // are zero and stay zero
+        constexpr int PER = (N == 64 ? 32 : N) / 2;
+#pragma unroll
+        for (int k = 0; k < PER; k++) {
+            const int i = g * PER + k;
+            x[i * P + v] = txfm_identity_one<N>(x[i * P + v]);
+        }
+    }
 }
 
 }  // namespace b200

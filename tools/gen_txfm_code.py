@@ -9,6 +9,16 @@ permutations) cost nothing.  Two pruned 64-point variants are emitted as well: F
 the 32 outputs the packed coefficient layout keeps (dead nodes dropped), IDCT64_in32 assumes inputs
 32..63 are zero (zero operands folded: half_btf with one zero operand is a single product).  Arithmetic is the reference's: 32-bit wrapping add/sub, half_btf with
 32-bit wrapping products summed in 64 bits (Source/Lib/Codec/inv_transforms.h:264).
+
+Lane splits of the 32- and 64-point DCTs (the ones the fused kernel runs: FDCT32, FDCT64_lo32, IDCT32, IDCT64_in32):
+the network's values after some stage fall into two groups whose cones share nothing but the inputs (which every
+lane reads from shared memory).  split_plan() finds them by slicing the graph: it takes the largest stage count
+`cut` at which the values fall into exactly two such groups.
+  cut == all stages (forward DCT: even / odd outputs): <name>_g0 / _g1 compute the outputs of one group each;
+  cut <  all stages (inverse DCT: the last stage combines the halves): <name>_g0 / _g1 compute the group's values
+  after stage `cut`, and <name>_t0 / _t1 run the remaining stages from the whole cut vector to the outputs whose
+  indices belong to that group.
+struct TxgSplit_<name> gathers them with the element masks (bit i: element i) of what each one writes.
 """
 import os
 import re
@@ -106,6 +116,83 @@ def emit(tag, n, stages, name=None, live_out=None, zero_in=None):
     return "\n".join(out)
 
 
+def split_plan(n, stages):
+    """(cut, [group0, group1]): see the module docstring.  Groups are sorted element-index lists."""
+    for cut in range(len(stages), 0, -1):
+        parent = {}
+
+        def find(v):
+            while parent.setdefault(v, v) != v:
+                v = parent[v]
+            return v
+
+        cur = [("in", i) for i in range(n)]
+        for s in range(cut):
+            new = []
+            for i, (btf, wa, a, wb, b, cl) in enumerate(stages[s]):
+                me = (s, i)
+                find(me)
+                for w, o in ((wa, a), (wb, b)):
+                    if w and cur[o][0] != "in":  # inputs are shared read-only leaves: they do not join groups
+                        parent[find(me)] = find(cur[o])
+                new.append(me)
+            cur = new
+        groups = {}
+        for i, v in enumerate(cur):
+            groups.setdefault(find(v), []).append(i)
+        if len(groups) >= 2:
+            assert len(groups) == 2, "split into %d groups" % len(groups)
+            return cut, sorted((sorted(g) for g in groups.values()), key=lambda g: g[0])
+    raise ValueError("network does not split")
+
+
+# the networks the fused kernel runs split across two lanes: (emitted name, graph tag, live outputs, zero inputs)
+SPLITS = (("FDCT32", "FDCT32", None, None),
+          ("FDCT64_lo32", "FDCT64", range(32), None),
+          ("IDCT32", "IDCT32", None, None),
+          ("IDCT64_in32", "IDCT64", None, set(range(32, 64))))
+
+
+def split_functions(n, stages, name, live_out=None, zero_in=None):
+    """[(function name, stage range, live outputs of the function)] of the split of one network"""
+    cut, groups = split_plan(n, stages)
+    live = set(range(n)) if live_out is None else set(live_out)
+    fns = []
+    for k, g in enumerate(groups):
+        if cut == len(stages):
+            fns.append(("%s_g%d" % (name, k), (0, cut), sorted(set(g) & live)))
+        else:
+            fns.append(("%s_g%d" % (name, k), (0, cut), list(g)))
+            fns.append(("%s_t%d" % (name, k), (cut, len(stages)), sorted(set(g) & live)))
+    return cut, fns
+
+
+def emit_split(n, stages, name, live_out=None, zero_in=None):
+    """the split's functions, then struct TxgSplit_<name>: kTail, the masks kMid<k> (what _g<k> writes) and kOut<k>
+    (the outputs lane group k stores), mid<k>() / tail<k>() dispatching to the functions"""
+    cut, fns = split_functions(n, stages, name, live_out, zero_in)
+    out = []
+    for fn, (s0, s1), live in fns:
+        out.append(emit(fn, n, stages[s0:s1], name=fn, live_out=live, zero_in=zero_in if s0 == 0 else None))
+        out.append("")
+    mask = {fn: "0x%016xull" % sum(1 << i for i in live) for fn, _, live in fns}
+    tail = cut < len(stages)
+    sig = "(int32_t (&x)[%d], const int32_t* __restrict__ cosv, const int cos_bit, const int clampb)" % n
+    out.append("struct TxgSplit_%s {" % name)
+    out.append("    static constexpr bool kTail = %s;" % ("true" if tail else "false"))
+    for k in range(2):
+        out.append("    static constexpr unsigned long long kMid%d = %s, kOut%d = %s;" %
+                   (k, mask["%s_g%d" % (name, k)], k, mask["%s_%s%d" % (name, "t" if tail else "g", k)]))
+    for part, letter in (("mid", "g"), ("tail", "t")) if tail else (("mid", "g"),):
+        out.append("    template <int G> static __device__ __forceinline__ void %s%s {" % (part, sig))
+        out.append("        if constexpr (G == 0) txg_%s_%s0(x, cosv, cos_bit, clampb); else txg_%s_%s1(x, cosv, cos_bit, clampb);" %
+                   (name, letter, name, letter))
+        out.append("    }")
+    out.append("};")
+    out.append("")
+    return "\n".join(out)
+
+
 def main():
     graphs = parse(SRC)
     parts = ["// GENERATED by tools/gen_txfm_code.py from txfm_graphs.inc -- do not edit.",
@@ -119,6 +206,11 @@ def main():
         if tag == "IDCT64":  # packed input: coefficients 32..63 are zero (inv_transforms.c:2567-2686)
             parts.append(emit(tag, n, stages, name="IDCT64_in32", zero_in=set(range(32, 64))))
             parts.append("")
+    by_tag = {tag: (n, stages) for tag, n, stages in graphs}
+    parts.append("// Two-lane splits (see tools/gen_txfm_code.py)")
+    for name, tag, live_out, zero_in in SPLITS:
+        n, stages = by_tag[tag]
+        parts.append(emit_split(n, stages, name, live_out, zero_in))
     open(DST, "w").write("\n".join(parts))
     print("wrote", DST, "(%d networks)" % len(graphs))
 
