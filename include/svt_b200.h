@@ -227,7 +227,7 @@ typedef struct SvtB200InvTxfmItem {
 SVT_B200_DECL_HANDLE(16x64) SVT_B200_DECL_HANDLE(32x64) SVT_B200_DECL_HANDLE(64x16) SVT_B200_DECL_HANDLE(64x32) SVT_B200_DECL_HANDLE(64x64)
 #undef SVT_B200_DECL_HANDLE
 
-/* A transform block is processed by a team of max(W,H) threads; its "team class" is
+/* A transform block is processed by a team of threads chosen by its "team class",
  * log2(max(W,H)) - 2 (0: 4x4 .. 4: the 64-point sizes).  Items must be ordered by class: the
  * n_per_class[0] class-0 items first, then class 1, ...; within a class, keeping equal (tx_size,
  * tx_type) together lets the teams that share a warp run in lock step. */

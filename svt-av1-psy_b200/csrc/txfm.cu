@@ -1,17 +1,22 @@
-// txfm.cu -- K5 forward 2-D transforms, K6 inverse 2-D transforms + reconstruction (sm_90a).
+// txfm.cu -- K5 forward 2-D transforms, K6 inverse 2-D transforms + reconstruction, and the fused chain of both
+// with the quantiser between them (sm_90a).
 //
 // Reference behaviour restated: av1_tranform_two_d_core_c (Source/Lib/Codec/transforms.c:2259-2324)
 // and inv_txfm2d_add_c (Source/Lib/Codec/inv_transforms.c:2459-2534), for all 19 transform sizes and
 // 16 transform types, 8/10/12-bit.  The 2-D configuration table (flips, per-pass kernel, cos_bit,
 // shifts) is dumped from the reference (txfm_cfg.inc); the 1-D networks are txfm_graphs.inc.
 //
-// H100 mapping: a team of max(W,H) threads per transform block (4, 8, 16, 32 or 64: the block's
-// "team class"), one thread per column in the column pass and one per row in the row pass, each
-// running the generated straight-line network on its vector in registers (txfm_tables.cuh).  The
-// block sits in shared memory in element-major order with an odd pitch, so the passes and the
-// transposing hand-over are bank-conflict free; residual loads / coefficient stores are coalesced rows.
+// H100 mapping: one kernel, txfm_kernel, whose modes are the forward batch, the inverse batch and the fused chain.
+// A transform block belongs to a team sized by its team class, log2(max(W,H)) - 2.  In the 4-, 8- and 16-point
+// classes a team is max(W,H) threads and several teams share a CTA: one thread per column in the column pass and one
+// per row in the row pass, each running the generated straight-line network on its vector in registers
+// (txfm_tables.cuh).  In the 32- and 64-point classes a block has a CTA of 2 * max(W,H) threads to itself, and its
+// 32- and 64-point vectors run split across two lanes.  The block sits in shared memory in element-major order with
+// an odd pitch, so the passes and the transposing hand-over are bank-conflict free; residual loads / coefficient
+// stores are coalesced rows.
 #include <map>
 #include <mutex>
+#include <type_traits>
 #include "txfm_tables.cuh"
 #include "quant_one.cuh"
 #include "../../include/svt_b200.h"
@@ -51,293 +56,238 @@ __host__ __device__ inline int rect_log_ratio(int w, int h) {  // get_rect_tx_lo
 }
 
 // ------------------------------------------------------------------------------------------------
-// forward
+// One block body for the three batch calls, as the modes of txfm_kernel:
+//   Forward (svt_b200_fwd_txfm_batch_dev): residual -> coefficients;
+//   Inverse (svt_b200_inv_txfm_batch_dev): dequantised coefficients + prediction -> reconstruction;
+//   Chain   (the fused calls): the per-block chain of the final encode pass (coding_loop.c:405-658), forward transform
+//           -> quantise -> inverse transform + reconstruction without leaving shared memory: the coefficients and the
+//           dequantised levels never travel through HBM between the steps.
+// The fused calls are bit-identical to the separate ones because each step is the same code in every mode.
 // ------------------------------------------------------------------------------------------------
-template <int TEAM, int THREADS>
-__global__ void __launch_bounds__(THREADS)
-fwd_txfm_kernel(const int16_t* __restrict__ src_base, int32_t* __restrict__ dst_base,
-                const SvtB200FwdTxfmItem* __restrict__ items, int n_items) {
-    extern __shared__ __align__(16) int32_t tsm[];
-    // a 64-point block is alone in its CTA: all THREADS move data, the first 64 run the passes
-    constexpr int TEAMS = TEAM >= 64 ? 1 : THREADS / TEAM, PLANE = TEAM * (TEAM + 1), MOVERS = TEAM >= 64 ? THREADS : TEAM;
-    const int     team  = TEAM >= 64 ? 0 : threadIdx.x / TEAM, tid = TEAM >= 64 ? threadIdx.x : threadIdx.x % TEAM;
-    int32_t*      A     = tsm + (size_t)team * team_stride(TEAM);
-    int32_t*      B     = A + PLANE;
+struct Forward { using Item = SvtB200FwdTxfmItem; };
+struct Inverse { using Item = SvtB200InvTxfmItem; };
+struct Chain { using Item = SvtB200TrioItem; };
 
-    for (int it = blockIdx.x * TEAMS + team; it < n_items; it += gridDim.x * TEAMS) {
-        const SvtB200FwdTxfmItem item = items[it];
-        const int   sz = item.tx_size, W = tx_w(sz), H = tx_h(sz);
-        const int   lgW = 31 - __clz(W);
-        const TxCfg cfg = c_txcfg[sz][item.tx_type];
-        const int16_t* src = src_base + item.src_off;
-        int32_t*       dst = dst_base + item.dst_off;
-        const int P1 = W + 1, P2 = H + 1;
-        const int part_shift = (item.reserved >> 1) & 3;  // 0 full, 1 = N2, 2 = N4
-        // load, optional up/down flip, pre-shift (transforms.c:2286-2294)
-        for (int idx = tid; idx < W * H; idx += MOVERS) {
-            const int r = idx >> lgW, c = idx & (W - 1);
-            const int rr = cfg.f_ud ? (H - 1 - r) : r;
-            A[r * P1 + c] = round_shift_arr((int32_t)src[(size_t)rr * item.src_stride + c], -cfg.f_s0);
-        }
-        team_sync<TEAM>();
-        txfm_pass_1d<TEAM, false>(cfg.f_tc, A, H, W, P1, cfg.f_cbc, 0, tid);  // columns: vector v = column v
-        team_sync<TEAM>();
-        // round-shift, optional left/right flip, hand over transposed (element = column)
-        for (int idx = tid; idx < W * H; idx += MOVERS) {
-            const int r = idx >> lgW, c = idx & (W - 1);
-            const int cc = cfg.f_lr ? (W - 1 - c) : c;
-            B[cc * P2 + r] = round_shift_arr(A[r * P1 + c], -cfg.f_s1);
-        }
-        team_sync<TEAM>();
-        txfm_pass_1d<TEAM, false>(cfg.f_tr, B, W, H, P2, cfg.f_cbr, 0, tid);  // rows: vector v = row v
-        team_sync<TEAM>();
-        const int rect = rect_log_ratio(W, H);
-        for (int idx = tid; idx < W * H; idx += MOVERS) {
-            const int r = idx >> lgW, c = idx & (W - 1);
-            int32_t   v = round_shift_arr(B[c * P2 + r], -cfg.f_s2);
-            if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewSqrt2, 12);
-            // N2 / N4 (av1_tranform_two_d_core_N2_c / _N4_c, transforms.c:5202, 6769): the top-left half / quarter
-            // of every dimension, identical to the full transform's values there, zero everywhere else
-            if (part_shift && (r >= max(H >> part_shift, 1) || c >= max(W >> part_shift, 1))) v = 0;
-            if (item.reserved & 1) {  // packed output: keep the top-left min(W,32) x min(H,32) (svt_handle_transform64x64 repack, transforms.c:2374)
-                const int Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;
-                if (r < Hp && c < Wp) dst[r * Wp + c] = v;
-            } else
-                dst[idx] = v;
-        }
-        team_sync<TEAM>();
-    }
+// the forward and the inverse part of an item: a Chain item has both, a Forward or an Inverse item is its own only part
+template <class I> __device__ __forceinline__ const I& fwd_part(const I& i) { return i; }
+template <class I> __device__ __forceinline__ const I& inv_part(const I& i) { return i; }
+__device__ __forceinline__ const SvtB200FwdTxfmItem& fwd_part(const SvtB200TrioItem& i) { return i.fwd; }
+__device__ __forceinline__ const SvtB200InvTxfmItem& inv_part(const SvtB200TrioItem& i) { return i.inv; }
+// the part that holds a block's tx_size and tx_type: a Chain item's forward part, otherwise the item itself
+template <class I> __device__ __forceinline__ const auto& shape_part(const I& i) { return fwd_part(i); }
+
+// the forward's last steps on one coefficient: final shift, then the scaling of 2:1 rectangles
+__device__ __forceinline__ int32_t fwd_out(int32_t v, const TxCfg& cfg, int rect) {
+    v = round_shift_arr(v, -cfg.f_s2);
+    if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewSqrt2, 12);
+    return v;
+}
+// the inverse's first steps on one dequantised coefficient: the scaling of 2:1 rectangles, then the row clamp
+__device__ __forceinline__ int32_t inv_in(int32_t v, int rect, int row_clamp) {
+    if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewInvSqrt2, 12);
+    return clamp_bits(v, row_clamp);
 }
 
-// ------------------------------------------------------------------------------------------------
-// inverse + reconstruction
-// ------------------------------------------------------------------------------------------------
-template <int TEAM, int THREADS, typename PIX>
-__global__ void __launch_bounds__(THREADS)
-inv_txfm_kernel(const int32_t* __restrict__ coef_base, const PIX* __restrict__ pred_base, PIX* __restrict__ recon_base,
-                const SvtB200InvTxfmItem* __restrict__ items, int n_items) {
-    extern __shared__ __align__(16) int32_t tsm[];
-    // a 64-point block is alone in its CTA: all THREADS move data, the first 64 run the passes
-    constexpr int TEAMS = TEAM >= 64 ? 1 : THREADS / TEAM, PLANE = TEAM * (TEAM + 1), MOVERS = TEAM >= 64 ? THREADS : TEAM;
-    const int     team  = TEAM >= 64 ? 0 : threadIdx.x / TEAM, tid = TEAM >= 64 ? threadIdx.x : threadIdx.x % TEAM;
-    int32_t*      A     = tsm + (size_t)team * team_stride(TEAM);
-    int32_t*      B     = A + PLANE;
-
-    for (int it = blockIdx.x * TEAMS + team; it < n_items; it += gridDim.x * TEAMS) {
-        const SvtB200InvTxfmItem item = items[it];
-        const int   sz = item.tx_size, W = tx_w(sz), H = tx_h(sz), bd = item.bd;
-        const int   lgW = 31 - __clz(W);
-        const TxCfg cfg = c_txcfg[sz][item.tx_type];
-        const int32_t* in = coef_base + item.coef_off;
-        const int Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;  // 64-point dims arrive packed (inv_transforms.c:2567-2686)
-        const int P1 = H + 1, P2 = W + 1;
-        const int rect = rect_log_ratio(W, H);
-        const int row_clamp = bd + 8;
-        const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
-        const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);  // svt_av1_gen_inv_stage_range
-        const int opt_col = bd == 12 ? 18 : 16;
-        // rows first: element = column, vector = row
-        for (int idx = tid; idx < W * H; idx += MOVERS) {
-            const int r = idx >> lgW, c = idx & (W - 1);
-            int32_t   v = (r < Hp && c < Wp) ? in[r * Wp + c] : 0;
-            if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewInvSqrt2, 12);
-            A[c * P1 + r] = clamp_bits(v, row_clamp);
-        }
-        team_sync<TEAM>();
-        txfm_pass_1d<TEAM, true>(cfg.i_tr, A, W, H, P1, cfg.i_cbr, opt_row, tid);
-        team_sync<TEAM>();
-        for (int idx = tid; idx < W * H; idx += MOVERS) {
-            const int r = idx >> lgW, c = idx & (W - 1);
-            const int cs = cfg.i_lr ? (W - 1 - c) : c;
-            B[r * P2 + c] = clamp_bits(round_shift_arr(A[cs * P1 + r], -cfg.i_s0), col_clamp);
-        }
-        team_sync<TEAM>();
-        txfm_pass_1d<TEAM, true>(cfg.i_tc, B, H, W, P2, cfg.i_cbc, opt_col, tid);
-        team_sync<TEAM>();
-        const PIX* pr = pred_base + item.pred_off;
-        PIX*       pw = recon_base + item.recon_off;
-        const long long int_max = (1ll << (7 + bd)) - 1 + (914ll << (bd - 7));  // check_range, inv_transforms.c:2401
-        const int       pix_max = (1 << bd) - 1;
-        for (int idx = tid; idx < W * H; idx += MOVERS) {
-            const int r = idx >> lgW, c = idx & (W - 1);
-            const int rs = cfg.i_ud ? (H - 1 - r) : r;
-            long long t  = (long long)round_shift_arr(B[rs * P2 + c], -cfg.i_s1);
-            t            = t < -int_max - 1 ? -int_max - 1 : (t > int_max ? int_max : t);
-            int p        = (int)pr[(size_t)r * item.pred_stride + c] + (int)t;
-            p            = p < 0 ? 0 : (p > pix_max ? pix_max : p);
-            pw[(size_t)r * item.recon_stride + c] = (PIX)p;
-        }
-        team_sync<TEAM>();
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// fused: forward transform -> quantise -> inverse transform + reconstruction of one block
-// (the per-block chain of the final encode pass, coding_loop.c:405-658) without leaving shared memory:
-// the coefficients and the dequantised levels never travel through HBM between the three steps.
-// ------------------------------------------------------------------------------------------------
-// the 1-D passes of the fused kernel: in the big-block classes (one block per CTA of 2 * TEAM threads) 32- and 64-point
-// vectors run split across two lanes, shorter ones one per thread
-template <int TEAM, int THREADS, bool INV>
-__device__ __forceinline__ void trio_pass(int type, int32_t* x, int N, int V, int P, int cos_bit, int clampb, int tid) {
+// A 1-D pass.  In the 32- and 64-point classes (one block per CTA of 2 * TEAM threads) 32- and 64-point vectors run split
+// across two lanes, shorter ones one per thread.  FULL64: 64-point vectors run whole on one thread, so that all 64 outputs
+// exist (the forward batch's unpacked items); otherwise the 64-point networks are the packed ones.
+template <int TEAM, int THREADS, bool INV, bool FULL64>
+__device__ __forceinline__ void txfm_pass(int type, int32_t* x, int N, int V, int P, int cos_bit, int clampb, int tid) {
     if constexpr (TEAM >= 32) {
         static_assert(THREADS == 2 * TEAM, "a lane pair per vector");
         if (N == 32) return txfm_pass_split<32, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
-        if constexpr (TEAM >= 64) {
+        if constexpr (TEAM >= 64 && !FULL64) {
             if (N == 64) return txfm_pass_split<64, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
         }
     }
-    txfm_pass_1d<TEAM, INV, true>(type, x, N, V, P, cos_bit, clampb, tid);
+    txfm_pass_1d<TEAM, INV, !FULL64>(type, x, N, V, P, cos_bit, clampb, tid);
 }
 
-template <int TEAM, int THREADS, typename PIX>
+template <class M, int TEAM, int THREADS, typename PIX>
 __global__ void __launch_bounds__(THREADS)
-trio_txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ srcpix_base /*non-null: residual = source - prediction, formed here*/,
-                 const PIX* __restrict__ pred_base, PIX* __restrict__ recon_base,
-                 int32_t* __restrict__ q_base, int32_t* __restrict__ dq_base /*may be null*/, const int16_t* __restrict__ iscan_base,
-                 const uint8_t* __restrict__ qm_base, const SvtB200TrioItem* __restrict__ items, int n_items,
-                 uint16_t* __restrict__ eobs) {
+txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ srcpix_base /*Chain, non-null: residual = source - prediction, formed here*/,
+            const PIX* __restrict__ pred_base, PIX* __restrict__ recon_base,
+            int32_t* __restrict__ coef_base /*Forward: the coefficients; Chain: the quantised levels*/,
+            int32_t* __restrict__ dq_base /*Chain: the dequantised levels, may be null*/, const int16_t* __restrict__ iscan_base,
+            const uint8_t* __restrict__ qm_base, const typename M::Item* __restrict__ items, int n_items, uint16_t* __restrict__ eobs,
+            const int32_t* __restrict__ dq_in /*Inverse: the dequantised coefficients*/) {
+    constexpr bool FWD = !std::is_same_v<M, Inverse>, INV = !std::is_same_v<M, Forward>, CHAIN = FWD && INV;
     extern __shared__ __align__(16) int32_t tsm[];
     // big blocks are few: one block per CTA (SOLO) of 2 * TEAM threads; all of them move its data, and lane pairs run
-    // its 32- and 64-point vectors (trio_pass)
+    // its 32- and 64-point vectors (txfm_pass)
     constexpr bool SOLO = TEAM >= 32;
     constexpr int  TEAMS = SOLO ? 1 : THREADS / TEAM, PLANE = TEAM * (TEAM + 1), MOVERS = SOLO ? THREADS : TEAM;
     const int      team  = SOLO ? 0 : threadIdx.x / TEAM, tid = SOLO ? threadIdx.x : threadIdx.x % TEAM;
-    int32_t*      A     = tsm + (size_t)team * team_stride(TEAM);
-    int32_t*      B     = A + PLANE;
+    int32_t*       A     = tsm + (size_t)team * team_stride(TEAM);
+    int32_t*       B     = A + PLANE;
     __shared__ int s_eob;
 
+    // a Forward or Inverse item is small and is copied into registers; a Chain item is read field by field where it is used
+    using ItemRef = std::conditional_t<CHAIN, const typename M::Item&, const typename M::Item>;
     for (int it = blockIdx.x * TEAMS + team; it < n_items; it += gridDim.x * TEAMS) {
-        const SvtB200TrioItem& item = items[it];
-        const int   sz = item.fwd.tx_size, W = tx_w(sz), H = tx_h(sz), bd = item.inv.bd;
+        const ItemRef item = items[it];
+        const auto& fi = fwd_part(item);
+        const int   sz = shape_part(item).tx_size, W = tx_w(sz), H = tx_h(sz);
         const int   lgW = 31 - __clz(W);
-        const TxCfg cfg = c_txcfg[sz][item.fwd.tx_type];
+        const TxCfg cfg = c_txcfg[sz][shape_part(item).tx_type];
         const int   rect = rect_log_ratio(W, H);
-        const int   Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;
-        {   // ---- forward (fwd_txfm_kernel) ----
-            const int P1 = W + 1, P2 = H + 1, sstride = item.fwd.src_stride;
-            if (srcpix_base) {  // svt_aom_residual_kernel fused in: the source picture shares the residual plane's geometry
-                const PIX* sp = srcpix_base + item.fwd.src_off;
-                const PIX* pp = pred_base + item.inv.pred_off;
-                const int  pstride = item.inv.pred_stride;
+        const int   Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;  // 64-point dimensions are packed (inv_transforms.c:2567-2686)
+        const int   PW = W + 1, PH = H + 1;  // odd pitches: a plane holds the block as [r * PW + c] or as [c * PH + r]
+        int         bd = 0;
+        if constexpr (INV) bd = inv_part(item).bd;
+        if constexpr (FWD) {  // ---- forward transform (transforms.c:2286-2318) ----
+            const int sstride = fi.src_stride;
+            // load, optional up/down flip, pre-shift
+            if constexpr (CHAIN) {
+                if (srcpix_base) {  // svt_aom_residual_kernel fused in: the source picture shares the residual plane's geometry
+                    const PIX* sp = srcpix_base + fi.src_off;
+                    const PIX* pp = pred_base + item.inv.pred_off;
+                    const int  pstride = item.inv.pred_stride;
 #pragma unroll 4
-                for (int idx = tid; idx < W * H; idx += MOVERS) {
-                    const int r = idx >> lgW, c = idx & (W - 1);
-                    const int rr = cfg.f_ud ? (H - 1 - r) : r;
-                    const int32_t d = (int32_t)sp[(size_t)rr * sstride + c] - (int32_t)pp[(size_t)rr * pstride + c];
-                    A[r * P1 + c] = round_shift_arr(d, -cfg.f_s0);
+                    for (int idx = tid; idx < W * H; idx += MOVERS) {
+                        const int r = idx >> lgW, c = idx & (W - 1);
+                        const int rr = cfg.f_ud ? (H - 1 - r) : r;
+                        const int32_t d = (int32_t)sp[(size_t)rr * sstride + c] - (int32_t)pp[(size_t)rr * pstride + c];
+                        A[r * PW + c] = round_shift_arr(d, -cfg.f_s0);
+                    }
                 }
-            } else {
-                const int16_t* src = src_base + item.fwd.src_off;
+            }
+            if (!CHAIN || !srcpix_base) {
+                const int16_t* src = src_base + fi.src_off;
 #pragma unroll 4
                 for (int idx = tid; idx < W * H; idx += MOVERS) {
                     const int r = idx >> lgW, c = idx & (W - 1);
                     const int rr = cfg.f_ud ? (H - 1 - r) : r;
-                    A[r * P1 + c] = round_shift_arr((int32_t)src[(size_t)rr * sstride + c], -cfg.f_s0);
+                    A[r * PW + c] = round_shift_arr((int32_t)src[(size_t)rr * sstride + c], -cfg.f_s0);
                 }
             }
             team_sync<TEAM, SOLO>();
-            trio_pass<TEAM, THREADS, false>(cfg.f_tc, A, H, W, P1, cfg.f_cbc, 0, tid);  // rows >= Hp of the result are not needed
+            // columns: vector v = column v (Chain: rows >= Hp of the result are not needed)
+            txfm_pass<TEAM, THREADS, false, !INV>(cfg.f_tc, A, H, W, PW, cfg.f_cbc, 0, tid);
             team_sync<TEAM, SOLO>();
+            // round-shift, optional left/right flip, hand over transposed (element = column); Chain: only the Hp rows that
+            // survive the packing
+            const int Hk = INV ? Hp : H;
 #pragma unroll 4
-            for (int idx = tid; idx < W * Hp; idx += MOVERS) {  // only the Hp rows that survive the packing
+            for (int idx = tid; idx < W * Hk; idx += MOVERS) {
                 const int r = idx >> lgW, c = idx & (W - 1);
                 const int cc = cfg.f_lr ? (W - 1 - c) : c;
-                B[cc * P2 + r] = round_shift_arr(A[r * P1 + c], -cfg.f_s1);
+                B[cc * PH + r] = round_shift_arr(A[r * PW + c], -cfg.f_s1);
             }
             team_sync<TEAM, SOLO>();
-            trio_pass<TEAM, THREADS, false>(cfg.f_tr, B, W, Hp, P2, cfg.f_cbr, 0, tid);
+            txfm_pass<TEAM, THREADS, false, !INV>(cfg.f_tr, B, W, Hk, PH, cfg.f_cbr, 0, tid);  // rows: vector v = row v
             team_sync<TEAM, SOLO>();
         }
-        int block_eob = 0;
-        {   // ---- quantise the (packed) coefficients; the dequantised levels become the inverse's input plane ----
-            const SvtB200QuantItem& qi = item.quant;
-            const uint8_t* qm  = qi.qm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.qm_off;
-            const uint8_t* iqm = qi.iqm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.iqm_off;
-            const int16_t* iscan = iscan_base + qi.scan_off;
-            int32_t*       qc = q_base + qi.q_off;
-            int32_t*       dqc = dq_base ? dq_base + qi.dq_off : nullptr;
-            const int P2 = H + 1, P1i = H + 1;  // forward result: B[c*P2 + r]; inverse input: A[c*P1i + r]
-            const int row_clamp = bd + 8;
-            if (SOLO && threadIdx.x == 0) s_eob = 0;
-            int eob = 0;
-#pragma unroll 4
+        if constexpr (!INV) {  // ---- Forward: the coefficients out ----
+            int32_t*  dst = coef_base + fi.dst_off;
+            const int part_shift = (fi.reserved >> 1) & 3;  // 0 full, 1 = N2, 2 = N4
             for (int idx = tid; idx < W * H; idx += MOVERS) {
                 const int r = idx >> lgW, c = idx & (W - 1);
-                int32_t   dq = 0;
-                if (r < Hp && c < Wp) {
-                    int32_t v = round_shift_arr(B[c * P2 + r], -cfg.f_s2);
-                    if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewSqrt2, 12);
-                    const int rc = r * Wp + c;
-                    int32_t   q;
-                    quant_one(qi, v, rc, qm, iqm, q, dq);
-                    qc[rc] = q;
-                    if (dqc) dqc[rc] = dq;
-                    if (q) eob = max(eob, (int)iscan[rc] + 1);
-                    if (rect == 1 || rect == -1) dq = round_shift64((long long)dq * kNewInvSqrt2, 12);
-                    dq = clamp_bits(dq, row_clamp);
-                }
-                A[c * P1i + r] = dq;  // rows first: element = column, vector = row
+                int32_t   v = fwd_out(B[c * PH + r], cfg, rect);
+                // N2 / N4 (av1_tranform_two_d_core_N2_c / _N4_c, transforms.c:5202, 6769): the top-left half / quarter
+                // of every dimension, identical to the full transform's values there, zero everywhere else
+                if (part_shift && (r >= max(H >> part_shift, 1) || c >= max(W >> part_shift, 1))) v = 0;
+                if (fi.reserved & 1) {  // packed output: keep the top-left min(W,32) x min(H,32) (svt_handle_transform64x64 repack, transforms.c:2374)
+                    if (r < Hp && c < Wp) dst[r * Wp + c] = v;
+                } else
+                    dst[idx] = v;
             }
-            if constexpr (SOLO) {
-                __syncthreads();
-                if (eob) atomicMax(&s_eob, eob);
-                __syncthreads();
-                eob = s_eob;
-                if (threadIdx.x == 0) eobs[it] = (uint16_t)eob;
-            } else {
-                const unsigned mask = TEAM == 32 ? 0xffffffffu : (((1u << TEAM) - 1u) << ((threadIdx.x & 31) / TEAM * TEAM));
-#pragma unroll
-                for (int o = TEAM / 2; o > 0; o >>= 1) eob = max(eob, __shfl_xor_sync(mask, eob, o));
-                if (tid == 0) eobs[it] = (uint16_t)eob;
-                team_sync<TEAM, SOLO>();
-            }
-            block_eob = eob;
-        }
-        if (block_eob == 0) {
-            // every level is zero: the inverse of an all-zero plane is zero, the reconstruction is the prediction
-            // (the encode pass takes the same shortcut, coding_loop.c: eob == 0 -> prediction copied); team-uniform branch
-            const PIX* pr = pred_base + item.inv.pred_off;
-            PIX*       pw = recon_base + item.inv.recon_off;
-            if (pr != pw) {
+            team_sync<TEAM, SOLO>();
+        } else {
+            // the inverse's input plane, rows first: A[c * PH + r], element = column, vector = row; zero outside the packed
+            // Wp x Hp, which the passes keep zero
+            const auto& ii = inv_part(item);
+            const int   row_clamp = bd + 8;
+            int eob = 0;
+            if constexpr (CHAIN) {  // ---- quantise the (packed) coefficients; the dequantised levels are the input ----
+                const SvtB200QuantItem& qi = item.quant;
+                const uint8_t* qm  = qi.qm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.qm_off;
+                const uint8_t* iqm = qi.iqm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.iqm_off;
+                const int16_t* iscan = iscan_base + qi.scan_off;
+                int32_t*       qc = coef_base + qi.q_off;
+                int32_t*       dqc = dq_base ? dq_base + qi.dq_off : nullptr;
+                if (SOLO && threadIdx.x == 0) s_eob = 0;
 #pragma unroll 4
                 for (int idx = tid; idx < W * H; idx += MOVERS) {
                     const int r = idx >> lgW, c = idx & (W - 1);
-                    pw[(size_t)r * item.inv.recon_stride + c] = pr[(size_t)r * item.inv.pred_stride + c];
+                    int32_t   dq = 0;
+                    if (r < Hp && c < Wp) {
+                        const int32_t v = fwd_out(B[c * PH + r], cfg, rect);
+                        const int     rc = r * Wp + c;
+                        int32_t       q;
+                        quant_one(qi, v, rc, qm, iqm, q, dq);
+                        qc[rc] = q;
+                        if (dqc) dqc[rc] = dq;
+                        if (q) eob = max(eob, (int)iscan[rc] + 1);
+                        dq = inv_in(dq, rect, row_clamp);
+                    }
+                    A[c * PH + r] = dq;
                 }
+                if constexpr (SOLO) {
+                    __syncthreads();
+                    if (eob) atomicMax(&s_eob, eob);
+                    __syncthreads();
+                    eob = s_eob;
+                    if (threadIdx.x == 0) eobs[it] = (uint16_t)eob;
+                } else {
+                    const unsigned mask = TEAM == 32 ? 0xffffffffu : (((1u << TEAM) - 1u) << ((threadIdx.x & 31) / TEAM * TEAM));
+#pragma unroll
+                    for (int o = TEAM / 2; o > 0; o >>= 1) eob = max(eob, __shfl_xor_sync(mask, eob, o));
+                    if (tid == 0) eobs[it] = (uint16_t)eob;
+                    team_sync<TEAM, SOLO>();
+                }
+            } else {  // ---- Inverse: the packed dequantised coefficients are the input ----
+                const int32_t* in = dq_in + ii.coef_off;
+                for (int idx = tid; idx < W * H; idx += MOVERS) {
+                    const int r = idx >> lgW, c = idx & (W - 1);
+                    A[c * PH + r] = (r < Hp && c < Wp) ? inv_in(in[r * Wp + c], rect, row_clamp) : 0;
+                }
+                team_sync<TEAM, SOLO>();
             }
-            team_sync<TEAM, SOLO>();
-        } else {   // ---- inverse + reconstruction (inv_txfm_kernel) ----
-            const int P1 = H + 1, P2 = W + 1;
-            const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
-            const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);
-            const int opt_col = bd == 12 ? 18 : 16;
-            trio_pass<TEAM, THREADS, true>(cfg.i_tr, A, W, Hp, P1, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
-            team_sync<TEAM, SOLO>();
+            if (CHAIN && eob == 0) {
+                // every level is zero: the inverse of an all-zero plane is zero, the reconstruction is the prediction
+                // (the encode pass takes the same shortcut, coding_loop.c: eob == 0 -> prediction copied); team-uniform branch
+                const PIX* pr = pred_base + ii.pred_off;
+                PIX*       pw = recon_base + ii.recon_off;
+                if (pr != pw) {
 #pragma unroll 4
-            for (int idx = tid; idx < W * H; idx += MOVERS) {
-                const int r = idx >> lgW, c = idx & (W - 1);
-                const int cs = cfg.i_lr ? (W - 1 - c) : c;
-                B[r * P2 + c] = clamp_bits(round_shift_arr(A[cs * P1 + r], -cfg.i_s0), col_clamp);
-            }
-            team_sync<TEAM, SOLO>();
-            trio_pass<TEAM, THREADS, true>(cfg.i_tc, B, H, W, P2, cfg.i_cbc, opt_col, tid);
-            team_sync<TEAM, SOLO>();
-            const PIX* pr = pred_base + item.inv.pred_off;
-            PIX*       pw = recon_base + item.inv.recon_off;
-            const long long int_max = (1ll << (7 + bd)) - 1 + (914ll << (bd - 7));
-            const int       pix_max = (1 << bd) - 1;
+                    for (int idx = tid; idx < W * H; idx += MOVERS) {
+                        const int r = idx >> lgW, c = idx & (W - 1);
+                        pw[(size_t)r * ii.recon_stride + c] = pr[(size_t)r * ii.pred_stride + c];
+                    }
+                }
+                team_sync<TEAM, SOLO>();
+            } else {  // ---- inverse transform + reconstruction (inv_transforms.c:2459-2534) ----
+                const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
+                const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);  // svt_av1_gen_inv_stage_range
+                const int opt_col = bd == 12 ? 18 : 16;
+                txfm_pass<TEAM, THREADS, true, false>(cfg.i_tr, A, W, Hp, PH, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
+                team_sync<TEAM, SOLO>();
 #pragma unroll 4
-            for (int idx = tid; idx < W * H; idx += MOVERS) {
-                const int r = idx >> lgW, c = idx & (W - 1);
-                const int rs = cfg.i_ud ? (H - 1 - r) : r;
-                long long t  = (long long)round_shift_arr(B[rs * P2 + c], -cfg.i_s1);
-                t            = t < -int_max - 1 ? -int_max - 1 : (t > int_max ? int_max : t);
-                int p        = (int)pr[(size_t)r * item.inv.pred_stride + c] + (int)t;
-                p            = p < 0 ? 0 : (p > pix_max ? pix_max : p);
-                pw[(size_t)r * item.inv.recon_stride + c] = (PIX)p;
+                for (int idx = tid; idx < W * H; idx += MOVERS) {
+                    const int r = idx >> lgW, c = idx & (W - 1);
+                    const int cs = cfg.i_lr ? (W - 1 - c) : c;
+                    B[r * PW + c] = clamp_bits(round_shift_arr(A[cs * PH + r], -cfg.i_s0), col_clamp);
+                }
+                team_sync<TEAM, SOLO>();
+                txfm_pass<TEAM, THREADS, true, false>(cfg.i_tc, B, H, W, PW, cfg.i_cbc, opt_col, tid);
+                team_sync<TEAM, SOLO>();
+                const PIX*      pr = pred_base + ii.pred_off;
+                PIX*            pw = recon_base + ii.recon_off;
+                const long long int_max = (1ll << (7 + bd)) - 1 + (914ll << (bd - 7));  // check_range, inv_transforms.c:2401
+                const int       pix_max = (1 << bd) - 1;
+#pragma unroll 4
+                for (int idx = tid; idx < W * H; idx += MOVERS) {
+                    const int r = idx >> lgW, c = idx & (W - 1);
+                    const int rs = cfg.i_ud ? (H - 1 - r) : r;
+                    long long t  = (long long)round_shift_arr(B[rs * PW + c], -cfg.i_s1);
+                    t            = t < -int_max - 1 ? -int_max - 1 : (t > int_max ? int_max : t);
+                    int p        = (int)pr[(size_t)r * ii.pred_stride + c] + (int)t;
+                    p            = p < 0 ? 0 : (p > pix_max ? pix_max : p);
+                    pw[(size_t)r * ii.recon_stride + c] = (PIX)p;
+                }
+                team_sync<TEAM, SOLO>();
             }
-            team_sync<TEAM, SOLO>();
         }
     }
 }
@@ -348,92 +298,62 @@ static inline int tx_class(int sz) {
     return m == 4 ? 0 : (m == 8 ? 1 : (m == 16 ? 2 : (m == 32 ? 3 : 4)));
 }
 
-template <typename K>
-static void set_smem_attr(K kernel, size_t smem) {
-    if (smem > 48 * 1024) B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-}
+// CTA size per team class: small enough that a picture's worth of blocks of that class spreads over all SMs.  A 32- or
+// 64-point block has its CTA of 2 * TEAM threads to itself (a lane pair per vector in the passes).
+template <int TEAM> constexpr int class_threads() { return TEAM >= 32 ? 2 * TEAM : (TEAM == 16 ? 128 : 256); }
 
-// CTA size per team class: small enough that a picture's worth of blocks of that class spreads over all SMs
-template <int TEAM> constexpr int class_threads() { return TEAM == 16 ? 128 : (TEAM == 32 ? 64 : 256); }
+// the device buffers of a batch call, in txfm_kernel's order; each mode uses its own
+struct TxfmBufs {
+    const int16_t* residual = nullptr;
+    const void*    source   = nullptr;
+    const void*    pred     = nullptr;
+    void*          recon    = nullptr;
+    int32_t*       coef     = nullptr;
+    int32_t*       dq       = nullptr;
+    const int16_t* iscan    = nullptr;
+    const uint8_t* qm       = nullptr;
+    const int32_t* dq_in    = nullptr;
+};
 
-template <int TEAM>
-static void launch_fwd_class(const int16_t* d_src, int32_t* d_dst, const SvtB200FwdTxfmItem* d_items, int n, cudaStream_t st) {
-    constexpr int    THREADS = class_threads<TEAM>(), TEAMS = TEAM >= 64 ? 1 : THREADS / TEAM;
+template <class M, int TEAM, typename PIX>
+static void launch(const TxfmBufs& b, const typename M::Item* items, int n, uint16_t* eobs, cudaStream_t st) {
+    if (n <= 0) return;
+    constexpr int    THREADS = class_threads<TEAM>(), TEAMS = TEAM >= 32 ? 1 : THREADS / TEAM;
     constexpr size_t smem = (size_t)TEAMS * team_stride(TEAM) * 4;
-    static int attr = -1;  // the initialisation (epoch) the attribute was applied in
-    if (attr != epoch()) { set_smem_attr(fwd_txfm_kernel<TEAM, THREADS>, smem); attr = epoch(); }
-    const int per_sm = (int)((200 * 1024) / (smem + 1024)) < 2048 / THREADS ? (int)((200 * 1024) / (smem + 1024)) : 2048 / THREADS;
-    fwd_txfm_kernel<TEAM, THREADS><<<grid_for((n + TEAMS - 1) / TEAMS, per_sm), THREADS, smem, st>>>(d_src, d_dst, d_items, n);
+    static_assert(smem <= 48 * 1024, "the default dynamic shared-memory limit: no attribute to set");
+    constexpr int per_sm = (int)((200 * 1024) / (smem + 1024)) < 2048 / THREADS ? (int)((200 * 1024) / (smem + 1024)) : 2048 / THREADS;
+    txfm_kernel<M, TEAM, THREADS, PIX><<<grid_for((n + TEAMS - 1) / TEAMS, per_sm), THREADS, smem, st>>>(
+        b.residual, (const PIX*)b.source, (const PIX*)b.pred, (PIX*)b.recon, b.coef, b.dq, b.iscan, b.qm, items, n, eobs, b.dq_in);
     B200_LAUNCH_CHECK();
 }
-void launch_fwd_txfm(const int16_t* d_src, int32_t* d_dst, const SvtB200FwdTxfmItem* d_items, int n, int cls, cudaStream_t st) {
-    if (n <= 0) return;
+// the n items of team class cls
+template <class M, typename PIX>
+static void launch_class(int cls, const TxfmBufs& b, const typename M::Item* items, int n, uint16_t* eobs, cudaStream_t st) {
     switch (cls) {
-    case 0: launch_fwd_class<4>(d_src, d_dst, d_items, n, st); break;
-    case 1: launch_fwd_class<8>(d_src, d_dst, d_items, n, st); break;
-    case 2: launch_fwd_class<16>(d_src, d_dst, d_items, n, st); break;
-    case 3: launch_fwd_class<32>(d_src, d_dst, d_items, n, st); break;
-    default: launch_fwd_class<64>(d_src, d_dst, d_items, n, st); break;
+    case 0: launch<M, 4, PIX>(b, items, n, eobs, st); break;
+    case 1: launch<M, 8, PIX>(b, items, n, eobs, st); break;
+    case 2: launch<M, 16, PIX>(b, items, n, eobs, st); break;
+    case 3: launch<M, 32, PIX>(b, items, n, eobs, st); break;
+    default: launch<M, 64, PIX>(b, items, n, eobs, st); break;
     }
 }
-
-template <int TEAM, typename PIX>
-static void launch_inv_class(const int32_t* d_coef, const PIX* d_pred, PIX* d_recon, const SvtB200InvTxfmItem* d_items, int n,
-                             cudaStream_t st) {
-    constexpr int    THREADS = class_threads<TEAM>(), TEAMS = TEAM >= 64 ? 1 : THREADS / TEAM;
-    constexpr size_t smem = (size_t)TEAMS * team_stride(TEAM) * 4;
-    static int attr = -1;  // the initialisation (epoch) the attribute was applied in
-    if (attr != epoch()) { set_smem_attr(inv_txfm_kernel<TEAM, THREADS, PIX>, smem); attr = epoch(); }
-    const int per_sm = (int)((200 * 1024) / (smem + 1024)) < 2048 / THREADS ? (int)((200 * 1024) / (smem + 1024)) : 2048 / THREADS;
-    inv_txfm_kernel<TEAM, THREADS, PIX><<<grid_for((n + TEAMS - 1) / TEAMS, per_sm), THREADS, smem, st>>>(d_coef, d_pred, d_recon, d_items, n);
-    B200_LAUNCH_CHECK();
-}
-template <typename PIX>
-void launch_inv_txfm(const int32_t* d_coef, const PIX* d_pred, PIX* d_recon, const SvtB200InvTxfmItem* d_items, int n, int cls,
-                     cudaStream_t st) {
-    if (n <= 0) return;
-    switch (cls) {
-    case 0: launch_inv_class<4, PIX>(d_coef, d_pred, d_recon, d_items, n, st); break;
-    case 1: launch_inv_class<8, PIX>(d_coef, d_pred, d_recon, d_items, n, st); break;
-    case 2: launch_inv_class<16, PIX>(d_coef, d_pred, d_recon, d_items, n, st); break;
-    case 3: launch_inv_class<32, PIX>(d_coef, d_pred, d_recon, d_items, n, st); break;
-    default: launch_inv_class<64, PIX>(d_coef, d_pred, d_recon, d_items, n, st); break;
-    }
-}
-
-template <int TEAM, typename PIX>
-static void launch_trio_class(const int16_t* d_src, const PIX* d_srcpix, const PIX* d_pred, PIX* d_recon, int32_t* d_q, int32_t* d_dq, const int16_t* d_iscan,
-                              const uint8_t* d_qm, const SvtB200TrioItem* d_items, int n, uint16_t* d_eobs, cudaStream_t st) {
-    if (n <= 0) return;
-    constexpr int    THREADS = TEAM >= 32 ? 2 * TEAM : class_threads<TEAM>(), TEAMS = TEAM >= 32 ? 1 : THREADS / TEAM;
-    constexpr size_t smem = (size_t)TEAMS * team_stride(TEAM) * 4;
-    static int attr = -1;  // the initialisation (epoch) the attribute was applied in
-    if (attr != epoch()) { set_smem_attr(trio_txfm_kernel<TEAM, THREADS, PIX>, smem); attr = epoch(); }
-    const int per_sm = (int)((200 * 1024) / (smem + 1024)) < 2048 / THREADS ? (int)((200 * 1024) / (smem + 1024)) : 2048 / THREADS;
-    trio_txfm_kernel<TEAM, THREADS, PIX><<<grid_for((n + TEAMS - 1) / TEAMS, per_sm), THREADS, smem, st>>>(d_src, d_srcpix, d_pred, d_recon, d_q, d_dq, d_iscan,
-                                                                                                     d_qm, d_items, n, d_eobs);
-    B200_LAUNCH_CHECK();
-}
-template <typename PIX>
-static void launch_trio(const int16_t* d_src, const PIX* d_srcpix, const PIX* d_pred, PIX* d_recon, int32_t* d_q, int32_t* d_dq, const int16_t* d_iscan,
-                        const uint8_t* d_qm, const SvtB200TrioItem* d_items, const int* n_per_class, uint16_t* d_eobs, cudaStream_t user) {
+// A batch ordered by class.  The five class launches are independent: the three big-block classes (few, long-running CTAs)
+// go to side streams forked from the caller's stream and joined back into it, so the many small blocks fill the SMs the
+// big ones leave idle.
+template <class M, typename PIX>
+static void launch_batch(const TxfmBufs& b, const typename M::Item* items, const int* n_per_class, uint16_t* eobs, cudaStream_t user) {
     int first[SVT_B200_TXFM_CLASSES + 1] = {0};
     for (int c = 0; c < SVT_B200_TXFM_CLASSES; c++) first[c + 1] = first[c] + n_per_class[c];
     ForkJoin& fj = fork_streams(user);
-    for (int c = SVT_B200_TXFM_CLASSES - 1; c >= 0; c--) {
-        cudaStream_t st = c >= 2 ? fj.side[c - 2] : user;
-        const SvtB200TrioItem* it = d_items + first[c];
-        uint16_t* eo = d_eobs + first[c];
-        const int n = n_per_class[c];
-        switch (c) {
-        case 0: launch_trio_class<4, PIX>(d_src, d_srcpix, d_pred, d_recon, d_q, d_dq, d_iscan, d_qm, it, n, eo, st); break;
-        case 1: launch_trio_class<8, PIX>(d_src, d_srcpix, d_pred, d_recon, d_q, d_dq, d_iscan, d_qm, it, n, eo, st); break;
-        case 2: launch_trio_class<16, PIX>(d_src, d_srcpix, d_pred, d_recon, d_q, d_dq, d_iscan, d_qm, it, n, eo, st); break;
-        case 3: launch_trio_class<32, PIX>(d_src, d_srcpix, d_pred, d_recon, d_q, d_dq, d_iscan, d_qm, it, n, eo, st); break;
-        default: launch_trio_class<64, PIX>(d_src, d_srcpix, d_pred, d_recon, d_q, d_dq, d_iscan, d_qm, it, n, eo, st); break;
-        }
-    }
+    for (int c = SVT_B200_TXFM_CLASSES - 1; c >= 0; c--)
+        launch_class<M, PIX>(c, b, items + first[c], n_per_class[c], eobs ? eobs + first[c] : nullptr, c >= 2 ? fj.side[c - 2] : user);
     join_streams(fj, user);
+}
+static bool class_counts_ok(const int* n_per_class) {
+    if (!n_per_class) return false;
+    for (int c = 0; c < SVT_B200_TXFM_CLASSES; c++)
+        if (n_per_class[c] < 0) return false;
+    return true;
 }
 
 }  // namespace b200
@@ -448,22 +368,14 @@ extern "C" int svt_b200_txfm_valid(int tx_size, int tx_type) {
 
 extern "C" int svt_b200_txfm_team_class(int tx_size) { return (tx_size < 0 || tx_size >= 19) ? -1 : tx_class(tx_size); }
 
-// The five class launches of a batch are independent: the three big-block classes (few, long-running
-// CTAs) go to side streams forked from the caller's stream and joined back into it, so the many
-// small blocks fill the SMs the big ones leave idle.
 extern "C" int svt_b200_fwd_txfm_batch_dev(const int16_t* d_residual, int32_t* d_coeff, const SvtB200FwdTxfmItem* d_items,
                                            const int n_per_class[SVT_B200_TXFM_CLASSES], void* stream) {
     require_ready();
-    if (!n_per_class) return SVT_B200_ERR_BAD_ARG;
-    int first[SVT_B200_TXFM_CLASSES + 1] = {0};
-    for (int c = 0; c < SVT_B200_TXFM_CLASSES; c++) {
-        if (n_per_class[c] < 0) return SVT_B200_ERR_BAD_ARG;
-        first[c + 1] = first[c] + n_per_class[c];
-    }
-    ForkJoin& fj = fork_streams((cudaStream_t)stream);
-    for (int c = SVT_B200_TXFM_CLASSES - 1; c >= 0; c--)
-        launch_fwd_txfm(d_residual, d_coeff, d_items + first[c], n_per_class[c], c, c >= 2 ? fj.side[c - 2] : (cudaStream_t)stream);
-    join_streams(fj, (cudaStream_t)stream);
+    if (!class_counts_ok(n_per_class)) return SVT_B200_ERR_BAD_ARG;
+    TxfmBufs b;
+    b.residual = d_residual;
+    b.coef     = d_coeff;
+    launch_batch<Forward, uint8_t>(b, d_items, n_per_class, nullptr, (cudaStream_t)stream);  // (the forward has no pixels)
     return SVT_B200_OK;
 }
 
@@ -471,19 +383,13 @@ extern "C" int svt_b200_inv_txfm_batch_dev(const int32_t* d_coeff, const void* d
                                            const SvtB200InvTxfmItem* d_items, const int n_per_class[SVT_B200_TXFM_CLASSES],
                                            int pixel_bytes, void* stream) {
     require_ready();
-    if (!n_per_class || (pixel_bytes != 1 && pixel_bytes != 2)) return SVT_B200_ERR_BAD_ARG;
-    int first[SVT_B200_TXFM_CLASSES + 1] = {0};
-    for (int c = 0; c < SVT_B200_TXFM_CLASSES; c++) {
-        if (n_per_class[c] < 0) return SVT_B200_ERR_BAD_ARG;
-        first[c + 1] = first[c] + n_per_class[c];
-    }
-    ForkJoin& fj = fork_streams((cudaStream_t)stream);
-    for (int c = SVT_B200_TXFM_CLASSES - 1; c >= 0; c--) {
-        cudaStream_t st = c >= 2 ? fj.side[c - 2] : (cudaStream_t)stream;
-        if (pixel_bytes == 1) launch_inv_txfm<uint8_t>(d_coeff, (const uint8_t*)d_pred, (uint8_t*)d_recon, d_items + first[c], n_per_class[c], c, st);
-        else launch_inv_txfm<uint16_t>(d_coeff, (const uint16_t*)d_pred, (uint16_t*)d_recon, d_items + first[c], n_per_class[c], c, st);
-    }
-    join_streams(fj, (cudaStream_t)stream);
+    if (!class_counts_ok(n_per_class) || (pixel_bytes != 1 && pixel_bytes != 2)) return SVT_B200_ERR_BAD_ARG;
+    TxfmBufs b;
+    b.pred  = d_pred;
+    b.recon = d_recon;
+    b.dq_in = d_coeff;
+    if (pixel_bytes == 1) launch_batch<Inverse, uint8_t>(b, d_items, n_per_class, nullptr, (cudaStream_t)stream);
+    else launch_batch<Inverse, uint16_t>(b, d_items, n_per_class, nullptr, (cudaStream_t)stream);
     return SVT_B200_OK;
 }
 
@@ -491,16 +397,11 @@ static int trio_entry(const int16_t* d_residual, const void* d_source, const voi
                       int32_t* d_dqcoeff, const int16_t* d_iscan, const uint8_t* d_qm, const SvtB200TrioItem* d_items,
                       const int n_per_class[SVT_B200_TXFM_CLASSES], uint16_t* d_eobs, int pixel_bytes, void* stream) {
     require_ready();
-    if (!n_per_class || !d_iscan || !d_qcoeff || !d_eobs || (pixel_bytes != 1 && pixel_bytes != 2)) return SVT_B200_ERR_BAD_ARG;
+    if (!class_counts_ok(n_per_class) || !d_iscan || !d_qcoeff || !d_eobs || (pixel_bytes != 1 && pixel_bytes != 2)) return SVT_B200_ERR_BAD_ARG;
     if (!d_residual == !d_source) return SVT_B200_ERR_BAD_ARG;  // exactly one of the two inputs
-    for (int c = 0; c < SVT_B200_TXFM_CLASSES; c++)
-        if (n_per_class[c] < 0) return SVT_B200_ERR_BAD_ARG;
-    if (pixel_bytes == 1)
-        launch_trio<uint8_t>(d_residual, (const uint8_t*)d_source, (const uint8_t*)d_pred, (uint8_t*)d_recon, d_qcoeff, d_dqcoeff, d_iscan, d_qm,
-                             d_items, n_per_class, d_eobs, (cudaStream_t)stream);
-    else
-        launch_trio<uint16_t>(d_residual, (const uint16_t*)d_source, (const uint16_t*)d_pred, (uint16_t*)d_recon, d_qcoeff, d_dqcoeff, d_iscan, d_qm,
-                              d_items, n_per_class, d_eobs, (cudaStream_t)stream);
+    const TxfmBufs b{d_residual, d_source, d_pred, d_recon, d_qcoeff, d_dqcoeff, d_iscan, d_qm};
+    if (pixel_bytes == 1) launch_batch<Chain, uint8_t>(b, d_items, n_per_class, d_eobs, (cudaStream_t)stream);
+    else launch_batch<Chain, uint16_t>(b, d_items, n_per_class, d_eobs, (cudaStream_t)stream);
     return SVT_B200_OK;
 }
 extern "C" int svt_b200_txfm_trio_batch_dev(const int16_t* d_residual, const void* d_pred, void* d_recon, int32_t* d_qcoeff,
@@ -701,15 +602,20 @@ extern "C" void svt_b200_fwd_txfm2d_partial(int16_t* input, int32_t* output, uin
     it->tx_type = (uint8_t)tx_type;
     it->reserved = (uint16_t)(level << 1);
     l->h2d(0, in_end);
-    launch_fwd_txfm(l->d<int16_t>(o_src), l->d<int32_t>(o_dst), l->d<SvtB200FwdTxfmItem>(o_it), 1, tx_class(tx_size), l->stream);
+    TxfmBufs b;
+    b.residual = l->d<int16_t>(o_src);
+    b.coef     = l->d<int32_t>(o_dst);
+    launch_class<Forward, uint8_t>(tx_class(tx_size), b, l->d<SvtB200FwdTxfmItem>(o_it), 1, nullptr, l->stream);
     l->d2h(o_dst, (size_t)W * H * 4);
     l->sync();
     memcpy(output, l->h<int32_t>(o_dst), (size_t)W * H * 4);
 }
 
-// ---- T1: svt_av1_inv_txfm2d_add_WxH (common_dsp_rtcd.h:106-142; C: inv_transforms.c:2545-2716) ----
-extern "C" void svt_b200_inv_txfm2d_add(const int32_t* input, uint16_t* output_r, int32_t stride_r, uint16_t* output_w,
-                                        int32_t stride_w, int tx_type, int tx_size, int32_t bd) {
+// ---- T1: svt_av1_inv_txfm2d_add_WxH (common_dsp_rtcd.h:106-142; C: inv_transforms.c:2545-2716) on 16-bit pixels, and
+// svt_b200_inv_txfm_add_8bit on 8-bit ones ----
+template <typename PIX>
+static void inv_txfm_add_t1(const int32_t* input, const PIX* pred, int32_t stride_r, PIX* out, int32_t stride_w, int tx_type,
+                            int tx_size, int bd) {
     require_ready();
     const int W = tx_w(tx_size), H = tx_h(tx_size);
     const int Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;
@@ -718,11 +624,11 @@ extern "C" void svt_b200_inv_txfm2d_add(const int32_t* input, uint16_t* output_r
         abort();
     }
     LaneGuard l;
-    size_t o_in = l->alloc((size_t)Wp * Hp * 4), o_pred = l->alloc((size_t)W * H * 2), o_it = l->alloc(sizeof(SvtB200InvTxfmItem));
+    size_t o_in = l->alloc((size_t)Wp * Hp * 4), o_pred = l->alloc((size_t)W * H * sizeof(PIX)), o_it = l->alloc(sizeof(SvtB200InvTxfmItem));
     size_t in_end = l->used;
-    size_t o_out = l->alloc((size_t)W * H * 2);
+    size_t o_out = l->alloc((size_t)W * H * sizeof(PIX));
     memcpy(l->h<int32_t>(o_in), input, (size_t)Wp * Hp * 4);
-    for (int r = 0; r < H; r++) memcpy(l->h<uint16_t>(o_pred) + r * W, output_r + (size_t)r * stride_r, W * 2);
+    for (int r = 0; r < H; r++) memcpy(l->h<PIX>(o_pred) + r * W, pred + (size_t)r * stride_r, W * sizeof(PIX));
     SvtB200InvTxfmItem* it = l->h<SvtB200InvTxfmItem>(o_it);
     memset(it, 0, sizeof(*it));
     it->pred_stride = it->recon_stride = W;
@@ -730,11 +636,22 @@ extern "C" void svt_b200_inv_txfm2d_add(const int32_t* input, uint16_t* output_r
     it->tx_type = (uint8_t)tx_type;
     it->bd = (uint8_t)bd;
     l->h2d(0, in_end);
-    launch_inv_txfm<uint16_t>(l->d<int32_t>(o_in), l->d<uint16_t>(o_pred), l->d<uint16_t>(o_out), l->d<SvtB200InvTxfmItem>(o_it), 1,
-                              tx_class(tx_size), l->stream);
-    l->d2h(o_out, (size_t)W * H * 2);
+    TxfmBufs b;
+    b.pred  = l->d<PIX>(o_pred);
+    b.recon = l->d<PIX>(o_out);
+    b.dq_in = l->d<int32_t>(o_in);
+    launch_class<Inverse, PIX>(tx_class(tx_size), b, l->d<SvtB200InvTxfmItem>(o_it), 1, nullptr, l->stream);
+    l->d2h(o_out, (size_t)W * H * sizeof(PIX));
     l->sync();
-    for (int r = 0; r < H; r++) memcpy(output_w + (size_t)r * stride_w, l->h<uint16_t>(o_out) + r * W, W * 2);
+    for (int r = 0; r < H; r++) memcpy(out + (size_t)r * stride_w, l->h<PIX>(o_out) + r * W, W * sizeof(PIX));
+}
+extern "C" void svt_b200_inv_txfm2d_add(const int32_t* input, uint16_t* output_r, int32_t stride_r, uint16_t* output_w,
+                                        int32_t stride_w, int tx_type, int tx_size, int32_t bd) {
+    inv_txfm_add_t1(input, output_r, stride_r, output_w, stride_w, tx_type, tx_size, bd);
+}
+extern "C" void svt_b200_inv_txfm_add_8bit(const int32_t* dqcoeff, uint8_t* dst_r, int32_t stride_r, uint8_t* dst_w,
+                                           int32_t stride_w, int tx_type, int tx_size) {
+    inv_txfm_add_t1(dqcoeff, dst_r, stride_r, dst_w, stride_w, tx_type, tx_size, 8);
 }
 
 // T2 host variants: caller-owned host planes, one call per batch.
@@ -756,8 +673,10 @@ extern "C" int svt_b200_fwd_txfm_batch_host(const int16_t* residual, size_t resi
     for (int c = 0, first = 0; c < SVT_B200_TXFM_CLASSES; first += cnt[c], c++) pos[c] = first;
     for (int i = 0; i < n_items; i++) hi[pos[tx_class(items[i].tx_size)]++] = items[i];
     l->h2d(0, in_end);
-    for (int c = 0, first = 0; c < SVT_B200_TXFM_CLASSES; first += cnt[c], c++)
-        launch_fwd_txfm(l->d<int16_t>(o_src), l->d<int32_t>(o_dst), l->d<SvtB200FwdTxfmItem>(o_it) + first, cnt[c], c, l->stream);
+    TxfmBufs b;
+    b.residual = l->d<int16_t>(o_src);
+    b.coef     = l->d<int32_t>(o_dst);
+    launch_batch<Forward, uint8_t>(b, l->d<SvtB200FwdTxfmItem>(o_it), cnt, nullptr, l->stream);
     l->d2h(o_dst, coeff_elems * 4);
     l->sync();
     // only the regions the items cover were written; copy those back
@@ -766,35 +685,6 @@ extern "C" int svt_b200_fwd_txfm_batch_host(const int16_t* residual, size_t resi
         memcpy(coeff + items[i].dst_off, l->h<int32_t>(o_dst) + items[i].dst_off, (size_t)W * H * 4);
     }
     return SVT_B200_OK;
-}
-
-extern "C" void svt_b200_inv_txfm_add_8bit(const int32_t* dqcoeff, uint8_t* dst_r, int32_t stride_r, uint8_t* dst_w,
-                                           int32_t stride_w, int tx_type, int tx_size) {
-    require_ready();
-    const int W = tx_w(tx_size), H = tx_h(tx_size);
-    const int Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;
-    if (!host_txcfg(tx_size, tx_type).valid) {
-        fprintf(stderr, "[svt_b200] FATAL: invalid (tx_size=%d, tx_type=%d)\n", tx_size, tx_type);
-        abort();
-    }
-    LaneGuard l;
-    size_t o_in = l->alloc((size_t)Wp * Hp * 4), o_pred = l->alloc((size_t)W * H), o_it = l->alloc(sizeof(SvtB200InvTxfmItem));
-    size_t in_end = l->used;
-    size_t o_out = l->alloc((size_t)W * H);
-    memcpy(l->h<int32_t>(o_in), dqcoeff, (size_t)Wp * Hp * 4);
-    for (int r = 0; r < H; r++) memcpy(l->h<uint8_t>(o_pred) + r * W, dst_r + (size_t)r * stride_r, W);
-    SvtB200InvTxfmItem* it = l->h<SvtB200InvTxfmItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->pred_stride = it->recon_stride = W;
-    it->tx_size = (uint8_t)tx_size;
-    it->tx_type = (uint8_t)tx_type;
-    it->bd = 8;
-    l->h2d(0, in_end);
-    launch_inv_txfm<uint8_t>(l->d<int32_t>(o_in), l->d<uint8_t>(o_pred), l->d<uint8_t>(o_out), l->d<SvtB200InvTxfmItem>(o_it), 1,
-                             tx_class(tx_size), l->stream);
-    l->d2h(o_out, (size_t)W * H);
-    l->sync();
-    for (int r = 0; r < H; r++) memcpy(dst_w + (size_t)r * stride_w, l->h<uint8_t>(o_out) + r * W, W);
 }
 
 // ---- T1: svt_handle_transform{16x64,32x64,64x16,64x32,64x64}{,_N2_N4} (aom_dsp_rtcd.h:216-240; C: transforms.c:2374-2543)

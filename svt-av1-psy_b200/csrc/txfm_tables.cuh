@@ -1,5 +1,5 @@
-// txfm_tables.cuh -- constant tables + the uniform 1-D butterfly evaluator shared by the forward
-// (txfm_fwd.cu) and inverse (txfm_inv.cu) 2-D transform kernels.
+// txfm_tables.cuh -- constant tables + the uniform 1-D butterfly evaluator of the 2-D transform kernel
+// (txfm.cu), in its forward, inverse and fused-chain modes.
 //
 // AV1's 1-D DCT/ADST are multi-stage butterfly networks with a rounding shift after every rotation
 // (reference: half_btf, Source/Lib/Codec/inv_transforms.h:264), so a GEMM cannot reproduce them
@@ -9,8 +9,8 @@
 // one thread holds one whole vector in registers -- stage permutations cost nothing and every
 // butterfly is a handful of integer instructions.  A team of max(W,H) threads owns a block: thread v
 // transforms column v, the block is handed over transposed through shared memory (odd pitch, so
-// both directions are bank-conflict free), then thread r transforms row r.  In the fused kernel's 32- and 64-point
-// classes a 32- or 64-point DCT vector is split across two lanes instead (txfm_pass_split).
+// both directions are bank-conflict free), then thread r transforms row r.  In the 32- and 64-point classes a 32- or
+// 64-point DCT vector is split across two lanes instead (txfm_pass_split).
 #pragma once
 #include <cstdint>
 #include "common.cuh"

@@ -333,7 +333,7 @@ class FramePipeline:
     # (call, stage it belongs to, the kernels it launches)
     CALLS = (("me_pyramid", "me", "downsample_2d_kernel+pad_plane_kernel"),
              ("me_search", "me", "me_b64_hme_kernel + fullpel_search_kernel + me_b64_finish_kernel"),
-             ("txfm_trio", "tx", "trio_txfm_kernel<4..64> (residual + forward transform + quantise + inverse transform fused)"),
+             ("txfm_trio", "tx", "txfm_kernel<Chain, 4..64> (residual + forward transform + quantise + inverse transform fused)"),
              ("pack_levels", "tx", "eob_chunk_sum_kernel+eob_offsets_kernel+pack_levels_kernel"),
              ("cdef_search", "cdef", "cdef_dir_kernel+cdef_search_kernel"),
              ("cdef_apply", "cdef", "cdef_apply_kernel"),

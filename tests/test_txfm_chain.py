@@ -194,13 +194,14 @@ def test_three_call_chain_matches_reference(b200, matrix, bd):
 
 
 def trio_grid_capacity(team):
-    """(CTAs per SM, teams per CTA) of the fused kernel's launch for one team class, as launch_trio_class (txfm.cu)
-    derives them: THREADS = 128 for the 32-point class, else class_threads (256, 256, 128, -, 256 for the 4- .. 64-point
-    classes); one team per CTA for the 32- and 64-point classes, THREADS / TEAM otherwise; dynamic shared memory =
-    teams * team_stride(TEAM) * 4 bytes; CTAs per SM = min(200 KB / (shared memory + 1 KB), 2048 / THREADS), and the grid
-    is min(CTAs needed, sm_count * CTAs per SM) (grid_for).  A class with more blocks than sm_count * CTAs per SM *
-    teams per CTA walks its grid-stride loop more than once."""
-    threads = 128 if team == 32 else {4: 256, 8: 256, 16: 128, 64: 256}[team]
+    """(CTAs per SM, teams per CTA) of one team class's launch, as launch (txfm.cu) derives them for all three modes of
+    txfm_kernel (the fused call and the separate forward and inverse calls): THREADS = class_threads (256, 256, 128 for
+    the 4- .. 16-point classes, 2 * TEAM = 64 and 128 for the 32- and 64-point classes); one team per CTA for the 32- and
+    64-point classes, THREADS / TEAM otherwise; dynamic shared memory = teams * team_stride(TEAM) * 4 bytes; CTAs per SM
+    = min(200 KB / (shared memory + 1 KB), 2048 / THREADS), and the grid is min(CTAs needed, sm_count * CTAs per SM)
+    (grid_for).  A class with more blocks than sm_count * CTAs per SM * teams per CTA walks its grid-stride loop more
+    than once."""
+    threads = 2 * team if team >= 32 else {4: 256, 8: 256, 16: 128}[team]
     teams = 1 if team >= 32 else threads // team
     stride = {4: 68, 8: 152, 16: 560}.get(team, 2 * team * (team + 1))
     smem = teams * stride * 4
@@ -210,7 +211,8 @@ def trio_grid_capacity(team):
 @gpu
 def test_grid_stride_loops_run_twice(b200, ref):
     """per class 2 x sm_count x CTAs per SM x teams per CTA blocks (+ a partial third pass): (8, 64), (8, 32), (10, 8),
-    (16, 1), (5, 1) CTAs per SM x teams per CTA for the 4- .. 64-point classes.  Fused and separate calls."""
+    (21, 1), (5, 1) CTAs per SM x teams per CTA for the 4- .. 64-point classes, so every CTA of every class loops at least
+    twice.  Fused and separate calls: they launch the same geometry."""
     import torch
     sms = int(b200.lib.svt_b200_sm_count())
     assert sms > 0
@@ -218,7 +220,7 @@ def test_grid_stride_loops_run_twice(b200, ref):
     for team in (4, 8, 16, 32, 64):
         per_sm, teams = trio_grid_capacity(team)
         counts.append(2 * sms * per_sm * teams + 37)
-    assert [trio_grid_capacity(t) for t in (4, 8, 16, 32, 64)] == [(8, 64), (8, 32), (10, 8), (16, 1), (5, 1)]
+    assert [trio_grid_capacity(t) for t in (4, 8, 16, 32, 64)] == [(8, 64), (8, 32), (10, 8), (21, 1), (5, 1)]
     r = rng(420)
     case = ch.build_case(ch.random_blocks(8, counts, r), 8, r, width=2048)
     assert case.n_per_class == counts

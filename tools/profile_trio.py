@@ -1,12 +1,13 @@
 #!/usr/bin/env python3
-"""Per-class timing of the fused transform chain (trio_txfm_kernel<4..64>) and the bench figures next to it.
+"""Per-class timing of the transform kernel (txfm_kernel<Chain / Forward / Inverse, 4..64>) and the bench figures next to it.
 
     python tools/profile_trio.py [--configs 1 2] [--steps 20] [--out DIR]
     python tools/profile_trio.py --bench-runs 3 --bench-trees . ../other_checkout [--bench-config 1]
 
 Profile mode: frames of each configuration through the hot path with every call in order on one stream, under
 torch.profiler (CUDA activities); one line per trio kernel -- name, grid, launches, mean us -- and the other calls'
-kernels summed per call, with the card's name and power limit.  The trace goes to DIR (default: a temporary
+kernels summed per call, with the card's name and power limit; then the separate calls (residual, forward, quantise,
+inverse) on the same frame, one line per forward and inverse kernel.  The traces go to DIR (default: a temporary
 directory).  Bench mode: `bench.py --gpus 1 --steps 3000 --warmup 50 --no-cpu-baseline` run alternately from each
 tree, `value` and `calls_ms` printed per run.  The two modes are separate processes: the profiler slows the host."""
 import argparse
@@ -52,20 +53,9 @@ def profile(configs, steps, out_dir):
                 fp.step(ev)  # with events: the calls run one after the other on the current stream
             torch.cuda.synchronize()
         prof.export_chrome_trace(trace)
-        kern = {}
-        for e in json.load(open(trace))["traceEvents"]:
-            if e.get("cat") != "kernel":
-                continue
-            name = e["name"]
-            short = name.split("(")[0].replace("void ", "").replace("b200::", "") or name[:60]
-            grid = tuple(e.get("args", {}).get("grid", ()))
-            k = kern.setdefault((short, grid), [0, 0.0])
-            k[0] += 1
-            k[1] += float(e["dur"])
+        kern = kernel_times(trace)
         print("config %d: %d profiled steps" % (cfg, steps))
-        trio = sorted(((s, g, n, t) for (s, g), (n, t) in kern.items() if "trio_txfm_kernel" in s), key=lambda x: -x[3] / x[2])
-        for s, g, n, t in trio:
-            print("  %-60s grid=%-14s launches=%-5d mean=%8.2f us" % (s, "x".join(map(str, g)), n, t / n))
+        print_classes(kern, "txfm_kernel<Chain")
         per = {}
         for (s, g), (n, t) in kern.items():
             base = s.split("<")[0]
@@ -75,7 +65,45 @@ def profile(configs, steps, out_dir):
         print("  all kernels, summed per name (us per step):")
         for base, (n, t) in sorted(per.items(), key=lambda x: -x[1][1]):
             print("    %-40s %8.2f" % (base, t / steps))
+        # the separate calls on the frame the steps left behind, in order on one stream
+        s = torch.cuda.current_stream().cuda_stream
+        calls = (fp.call_residual, fp.call_fwd_txfm, fp.call_quant, fp.call_inv_txfm)
+        for c in calls:
+            c(s)
+        torch.cuda.synchronize()
+        trace = os.path.join(out_dir, "separate_config%d.pt.trace.json" % cfg)
+        with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(steps):
+                for c in calls:
+                    c(s)
+            torch.cuda.synchronize()
+        prof.export_chrome_trace(trace)
+        kern = kernel_times(trace)
+        print("config %d: separate calls, %d profiled rounds" % (cfg, steps))
+        print_classes(kern, "txfm_kernel<Forward")
+        print_classes(kern, "txfm_kernel<Inverse")
         sys.stdout.flush()
+
+
+def kernel_times(trace):
+    """(short name, grid) -> [launches, total us] of the kernels in a chrome trace"""
+    kern = {}
+    for e in json.load(open(trace))["traceEvents"]:
+        if e.get("cat") != "kernel":
+            continue
+        name = e["name"]
+        short = name.split("(")[0].replace("void ", "").replace("b200::", "") or name[:60]
+        grid = tuple(e.get("args", {}).get("grid", ()))
+        k = kern.setdefault((short, grid), [0, 0.0])
+        k[0] += 1
+        k[1] += float(e["dur"])
+    return kern
+
+
+def print_classes(kern, prefix):
+    rows = sorted(((s, g, n, t) for (s, g), (n, t) in kern.items() if s.startswith(prefix)), key=lambda x: -x[3] / x[2])
+    for s, g, n, t in rows:
+        print("  %-60s grid=%-14s launches=%-5d mean=%8.2f us" % (s, "x".join(map(str, g)), n, t / n))
 
 
 def bench(trees, runs, config, steps, warmup):
