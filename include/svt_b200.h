@@ -475,6 +475,60 @@ SVT_B200_API int svt_b200_cdef_apply_frame_dev(const SvtB200CdefFrame* frame, co
                                                int out_stride_c, void* stream);
 
 /* ------------------------------------------------------------------------------------------ */
+/* K14  deblocking loop filter  (reference: deblocking_common.c:242-866, deblocking_filter.c:144-654) */
+/* ------------------------------------------------------------------------------------------ */
+/* T1: common_dsp_rtcd.h:1036-1067.  Each call filters 4 pixels along one edge at `s` (the first pixel on the q side):
+ * _4 / _6 / _8 / _14 read 2 / 3 / 4 / 7 pixels on each side of the edge and write 2 / 2 / 3 / 6.  Only blimit[0],
+ * limit[0] and thresh[0] are read.  High-bit-depth pixels are plain uint16_t*. */
+#define SVT_B200_DECL_LPF(DIR, N)                                                                                          \
+    SVT_B200_API void svt_b200_aom_lpf_##DIR##_##N(uint8_t* s, int32_t pitch, const uint8_t* blimit, const uint8_t* limit, \
+                                                   const uint8_t* thresh);                                                 \
+    SVT_B200_API void svt_b200_aom_highbd_lpf_##DIR##_##N(uint16_t* s, int32_t pitch, const uint8_t* blimit,               \
+                                                          const uint8_t* limit, const uint8_t* thresh, int32_t bd);
+SVT_B200_DECL_LPF(horizontal, 4) SVT_B200_DECL_LPF(horizontal, 6) SVT_B200_DECL_LPF(horizontal, 8) SVT_B200_DECL_LPF(horizontal, 14)
+SVT_B200_DECL_LPF(vertical, 4) SVT_B200_DECL_LPF(vertical, 6) SVT_B200_DECL_LPF(vertical, 8) SVT_B200_DECL_LPF(vertical, 14)
+#undef SVT_B200_DECL_LPF
+
+/* One record per 4x4 luma position of the picture's mode-info grid (ModeInfo.mbmi.block_mi, block_structures.h:108):
+ * the fields the edge derivation reads.  bsize = BlockSize, mode = PredictionMode, ref_frame0 = MvReferenceFrame
+ * (0 = INTRA_FRAME, 1..7 = LAST..ALTREF). */
+typedef struct SvtB200DlfMi {
+    uint8_t bsize;
+    uint8_t tx_depth;
+    uint8_t skip;
+    int8_t  ref_frame0;
+    uint8_t mode;
+    uint8_t segment_id;
+    uint8_t reserved[2];
+} SvtB200DlfMi;
+
+/* The picture and the frame's loop-filter state.  Pixels are uint8 (pixel_bytes 1: the 8-bit filters) or uint16
+ * (pixel_bytes 2: the high-bit-depth filters at bit_depth, 8 included).  4:2:0 only.  lvl and lfthr are the
+ * LoopFilterInfoN (definitions.h:1913-1922) that svt_av1_loop_filter_frame_init derives from the frame header on the host;
+ * lfthr[level] = {mblim, lim, hev_thr}. */
+typedef struct SvtB200DlfFrame {
+    void*   plane[3];       /* DEVICE pointers to pixel (0, 0) of Y, Cb, Cr */
+    int32_t stride[3];      /* in pixels */
+    int32_t width, height;  /* luma, unpadded: edges at x >= width (chroma: width >> 1) or y >= height are not filtered */
+    int32_t mi_rows, mi_cols, mi_stride; /* the record grid: at least ((height + 7) & ~7) / 4 rows, ((width + 7) & ~7) / 4 columns */
+    int32_t bit_depth;
+    int32_t pixel_bytes;
+    int32_t filter_level[2]; /* luma vertical / horizontal edges: both 0 = nothing is filtered, chroma included */
+    int32_t filter_level_u, filter_level_v; /* 0 = that plane is not filtered */
+    int32_t reserved;
+    uint8_t lvl[3][8][2][8][2]; /* [plane][segment][dir: 0 vertical edges, 1 horizontal][ref_frame0][mode delta index] */
+    uint8_t lfthr[64][3];
+    uint8_t reserved2[4];
+} SvtB200DlfFrame;
+
+/* T2: svt_av1_loop_filter_frame (deblocking_filter.c:625) over all three planes, in place: one pass over every vertical
+ * edge, then one over every horizontal edge (no edge reads a pixel another edge of its direction writes, so this equals
+ * the reference's superblock order).  d_mi: DEVICE array of mi_rows x mi_stride records.  Filtering reads and writes up
+ * to 7 pixels past the plane's width and height at edges that start inside it: the planes need that much readable and
+ * writable padding (the reference's recon pictures have it).  Returns SVT_B200_ERR_BAD_ARG for an inconsistent frame. */
+SVT_B200_API int svt_b200_loop_filter_frame_dev(const SvtB200DlfFrame* frame, const SvtB200DlfMi* d_mi, void* stream);
+
+/* ------------------------------------------------------------------------------------------ */
 /* K9/K11  Wiener filter + statistics  (reference: convolve.c:100-237, restoration_pick.c:659) */
 /* ------------------------------------------------------------------------------------------ */
 typedef struct SvtB200ConvolveParams { /* layout of ConvolveParams, Source/Lib/Codec/definitions.h:572-585 */

@@ -196,6 +196,24 @@ int svt_b200_install_rtcd(int device) {
     BIND(svt_av1_lowbd_pixel_proj_error, b200_lowbd_pixel_proj_error);
     BIND(svt_av1_highbd_pixel_proj_error, b200_highbd_pixel_proj_error);
     BIND(svt_get_proj_subspace, b200_get_proj_subspace);
+    GROUP(256u);
+    /* K14: deblocking loop filter (common_dsp_rtcd.h:1036-1067; the high-bit-depth pointers take real uint16_t addresses) */
+    BIND(svt_aom_lpf_horizontal_4, svt_b200_aom_lpf_horizontal_4);
+    BIND(svt_aom_lpf_horizontal_6, svt_b200_aom_lpf_horizontal_6);
+    BIND(svt_aom_lpf_horizontal_8, svt_b200_aom_lpf_horizontal_8);
+    BIND(svt_aom_lpf_horizontal_14, svt_b200_aom_lpf_horizontal_14);
+    BIND(svt_aom_lpf_vertical_4, svt_b200_aom_lpf_vertical_4);
+    BIND(svt_aom_lpf_vertical_6, svt_b200_aom_lpf_vertical_6);
+    BIND(svt_aom_lpf_vertical_8, svt_b200_aom_lpf_vertical_8);
+    BIND(svt_aom_lpf_vertical_14, svt_b200_aom_lpf_vertical_14);
+    BIND(svt_aom_highbd_lpf_horizontal_4, svt_b200_aom_highbd_lpf_horizontal_4);
+    BIND(svt_aom_highbd_lpf_horizontal_6, svt_b200_aom_highbd_lpf_horizontal_6);
+    BIND(svt_aom_highbd_lpf_horizontal_8, svt_b200_aom_highbd_lpf_horizontal_8);
+    BIND(svt_aom_highbd_lpf_horizontal_14, svt_b200_aom_highbd_lpf_horizontal_14);
+    BIND(svt_aom_highbd_lpf_vertical_4, svt_b200_aom_highbd_lpf_vertical_4);
+    BIND(svt_aom_highbd_lpf_vertical_6, svt_b200_aom_highbd_lpf_vertical_6);
+    BIND(svt_aom_highbd_lpf_vertical_8, svt_b200_aom_highbd_lpf_vertical_8);
+    BIND(svt_aom_highbd_lpf_vertical_14, svt_b200_aom_highbd_lpf_vertical_14);
     return SVT_B200_OK;
 }
 

@@ -321,6 +321,35 @@ def cdef_frame_desc(rec, src, width, height, bit_depth, damping, subsampling):
     return f
 
 # ------------------------------------------------------------------------------------------------
+# K14 deblocking loop filter
+# ------------------------------------------------------------------------------------------------
+LPF_TAPS = (4, 6, 8, 14)
+for _d in ("horizontal", "vertical"):
+    for _n in LPF_TAPS:
+        _f = getattr(lib, "svt_b200_aom_lpf_%s_%d" % (_d, _n))
+        _f.argtypes = [vp, ct.c_int32, vp, vp, vp]
+        _f.restype = None
+        _f = getattr(lib, "svt_b200_aom_highbd_lpf_%s_%d" % (_d, _n))
+        _f.argtypes = [vp, ct.c_int32, vp, vp, vp, ct.c_int32]
+        _f.restype = None
+lib.svt_b200_loop_filter_frame_dev.argtypes = [ct.POINTER(DlfFrame), vp, vp]
+lib.svt_b200_loop_filter_frame_dev.restype = ct.c_int
+
+
+def svt_aom_lpf(direction, taps, buf, offset, pitch, blimit, limit, thresh, bd=None):
+    """svt_aom_{,highbd_}lpf_<direction>_<taps> on a numpy buffer (uint8, or uint16 with bd) at element `offset`, in place"""
+    hb = buf.dtype == np.uint16
+    name = "svt_b200_aom_%slpf_%s_%d" % ("highbd_" if hb else "", direction, taps)
+    th = [np.full(16, v, np.uint8) for v in (blimit, limit, thresh)]
+    args = [_ptr(buf, byte_off=offset * buf.itemsize), pitch] + [_ptr(t) for t in th] + ([bd] if hb else [])
+    getattr(lib, name)(*args)
+
+
+def loop_filter_frame_dev(frame, d_mi, stream=0):
+    """svt_b200_loop_filter_frame_dev: frame = DlfFrame with device plane pointers, d_mi = device records (data pointer)"""
+    return lib.svt_b200_loop_filter_frame_dev(ct.byref(frame), vp(d_mi), vp(stream))
+
+# ------------------------------------------------------------------------------------------------
 # K9 / K11 Wiener
 # ------------------------------------------------------------------------------------------------
 lib.svt_b200_av1_wiener_convolve_add_src.argtypes = [vp, ct.c_ssize_t, vp, ct.c_ssize_t, vp, vp, ct.c_int32, ct.c_int32,

@@ -106,6 +106,22 @@ class CdefFrame(ct.Structure):
                      "damping", "subsampling_factor", "reserved")
 
 
+# ---- K14 deblocking loop filter ---------------------------------------------------------------------------------------
+class DlfMi(ct.Structure):
+    _fields_ = _same(ct.c_uint8, "bsize", "tx_depth", "skip") + [("ref_frame0", ct.c_int8), ("mode", ct.c_uint8), ("segment_id", ct.c_uint8),
+                                                                 ("reserved", ct.c_uint8 * 2)]
+
+
+class DlfFrame(ct.Structure):
+    _fields_ = [("plane", ct.c_void_p * 3), ("stride", ct.c_int32 * 3)] + \
+               _same(ct.c_int32, "width", "height", "mi_rows", "mi_cols", "mi_stride", "bit_depth", "pixel_bytes") + \
+               [("filter_level", ct.c_int32 * 2)] + _same(ct.c_int32, "filter_level_u", "filter_level_v", "reserved") + \
+               [("lvl", ct.c_uint8 * 2 * 8 * 2 * 8 * 3), ("lfthr", ct.c_uint8 * 3 * 64), ("reserved2", ct.c_uint8 * 4)]
+
+
+DLF_MI_DTYPE = np.dtype(DlfMi)
+
+
 # ---- K9/K11 Wiener filter + statistics, K10/K12 self-guided filter, a13 loop-restoration drivers --------------------
 class ConvolveParams(ct.Structure):  # == the reference's ConvolveParams
     _fields_ = [("ref", ct.c_int32), ("do_average", ct.c_int32), ("dst", ct.c_void_p)] + \
