@@ -528,6 +528,31 @@ typedef struct SvtB200DlfFrame {
  * writable padding (the reference's recon pictures have it).  Returns SVT_B200_ERR_BAD_ARG for an inconsistent frame. */
 SVT_B200_API int svt_b200_loop_filter_frame_dev(const SvtB200DlfFrame* frame, const SvtB200DlfMi* d_mi, void* stream);
 
+/* The trial costs of the filter-level search (search_filter_level, deblocking_filter.c:886): for each listed base level, the
+ * SSE against the source of one plane filtered at that level alone, as try_filter_frame (:840) measures it.  The host keeps
+ * the search itself and looks the costs up instead of filtering. */
+typedef struct SvtB200DlfLevelSse {
+    const void*    src[3];        /* DEVICE: source planes at pixel (0, 0), same pixel type as the recon planes */
+    int32_t        src_stride[3]; /* in pixels */
+    int32_t        sse_width, sse_height; /* luma SSE region (ppcs->aligned_width x aligned_height, at most
+                                             ((width + 7) & ~7) x ((height + 7) & ~7)); chroma: >> 1 */
+    int32_t        plane_mask;    /* bit p: evaluate plane p */
+    int32_t        n_levels;      /* 1..64 */
+    uint8_t        level[64];     /* base level of entry i (0..63); 0 = the plane unfiltered */
+    uint8_t        reserved[4];
+    const uint8_t* d_lvl;         /* DEVICE [3][n_levels][8][2][8][2]: lf_info.lvl[plane] as svt_av1_loop_filter_frame_init
+                                     derives it for level[i] (luma: both directions at level[i]); not read for level 0 */
+} SvtB200DlfLevelSse;
+
+/* T2: d_sse[p * n_levels + i] = try_filter_frame(level[i], plane p) for every plane p in the mask (other entries are not
+ * written).  From `frame` the call uses the recon planes, the geometry, bit_depth, pixel_bytes and lfthr (which must
+ * reflect the sharpness the search runs at), not filter_level* or lvl.  A chroma entry filters its plane whatever the
+ * frame's luma levels are, as the search does.  The recon planes are read, never written; no pixel left of or above
+ * (0, 0) or more than 7 past the plane's width or height is read.  d_mi: as for svt_b200_loop_filter_frame_dev.
+ * Returns SVT_B200_ERR_BAD_ARG for an inconsistent frame or level list, an empty mask or a missing plane. */
+SVT_B200_API int svt_b200_dlf_level_sse_dev(const SvtB200DlfFrame* frame, const SvtB200DlfLevelSse* s, const SvtB200DlfMi* d_mi,
+                                           int64_t* d_sse, void* stream);
+
 /* ------------------------------------------------------------------------------------------ */
 /* K9/K11  Wiener filter + statistics  (reference: convolve.c:100-237, restoration_pick.c:659) */
 /* ------------------------------------------------------------------------------------------ */

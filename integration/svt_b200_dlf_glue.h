@@ -25,4 +25,17 @@ struct EbPictureBufferDesc;
 int svt_b200_dlf_frame_from_pcs(const struct PictureControlSet* pcs, const struct EbPictureBufferDesc* recon, SvtB200DlfFrame* frame,
                                 SvtB200DlfMi* mi);
 
+/* For the filter-level search (search_filter_level, deblocking_filter.c:886), with svt_av1_loop_filter_init already run and
+ * the frame header's sharpness set, as svt_av1_pick_filter_level does before its first try: fills *frame as
+ * svt_b200_dlf_frame_from_pcs does (lfthr at the frame header's sharpness), *s with the source planes the search compares
+ * with (ppcs->enhanced_pic, or pcs->input_frame16bit in the 16-bit pipeline) at their visible origin, the SSE region
+ * (ppcs->aligned_width x aligned_height), plane_mask and the n_levels levels, and lvl[3][n_levels][8][2][8][2] with
+ * the table svt_av1_loop_filter_frame_init derives for each level of each plane in the mask (luma: both directions at the
+ * level; zeros for level 0).  Works on copies of the frame header and lf_info: the pcs is not changed.  The caller copies
+ * lvl to the device and sets s->d_lvl, and replaces the host plane pointers with the device copies.  Returns
+ * SVT_B200_ERR_BAD_ARG for what svt_b200_dlf_frame_from_pcs refuses, a bad level list or mask, or a missing source. */
+int svt_b200_dlf_level_sse_from_pcs(const struct PictureControlSet* pcs, const struct EbPictureBufferDesc* recon, int plane_mask,
+                                    int n_levels, const uint8_t* levels, SvtB200DlfFrame* frame, SvtB200DlfLevelSse* s,
+                                    uint8_t* lvl);
+
 #endif /* SVT_B200_DLF_GLUE_H */

@@ -334,6 +334,8 @@ for _d in ("horizontal", "vertical"):
         _f.restype = None
 lib.svt_b200_loop_filter_frame_dev.argtypes = [ct.POINTER(DlfFrame), vp, vp]
 lib.svt_b200_loop_filter_frame_dev.restype = ct.c_int
+lib.svt_b200_dlf_level_sse_dev.argtypes = [ct.POINTER(DlfFrame), ct.POINTER(DlfLevelSse), vp, vp, vp]
+lib.svt_b200_dlf_level_sse_dev.restype = ct.c_int
 
 
 def svt_aom_lpf(direction, taps, buf, offset, pitch, blimit, limit, thresh, bd=None):
@@ -348,6 +350,12 @@ def svt_aom_lpf(direction, taps, buf, offset, pitch, blimit, limit, thresh, bd=N
 def loop_filter_frame_dev(frame, d_mi, stream=0):
     """svt_b200_loop_filter_frame_dev: frame = DlfFrame with device plane pointers, d_mi = device records (data pointer)"""
     return lib.svt_b200_loop_filter_frame_dev(ct.byref(frame), vp(d_mi), vp(stream))
+
+
+def dlf_level_sse_dev(frame, s, d_mi, d_sse, stream=0):
+    """svt_b200_dlf_level_sse_dev: frame = DlfFrame, s = DlfLevelSse (device source planes and d_lvl), d_mi = device records,
+    d_sse = device int64 [3 * s.n_levels] (data pointers)"""
+    return lib.svt_b200_dlf_level_sse_dev(ct.byref(frame), ct.byref(s), vp(d_mi), vp(d_sse), vp(stream))
 
 # ------------------------------------------------------------------------------------------------
 # K9 / K11 Wiener

@@ -119,6 +119,12 @@ class DlfFrame(ct.Structure):
                [("lvl", ct.c_uint8 * 2 * 8 * 2 * 8 * 3), ("lfthr", ct.c_uint8 * 3 * 64), ("reserved2", ct.c_uint8 * 4)]
 
 
+class DlfLevelSse(ct.Structure):
+    _fields_ = [("src", ct.c_void_p * 3), ("src_stride", ct.c_int32 * 3)] + \
+               _same(ct.c_int32, "sse_width", "sse_height", "plane_mask", "n_levels") + \
+               [("level", ct.c_uint8 * 64), ("reserved", ct.c_uint8 * 4), ("d_lvl", ct.c_void_p)]
+
+
 DLF_MI_DTYPE = np.dtype(DlfMi)
 
 
