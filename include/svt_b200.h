@@ -706,8 +706,8 @@ SVT_B200_API int svt_b200_lr_filter_frame_dev(const SvtB200LrPlane* planes, int 
 SVT_B200_API int svt_b200_lr_unit_sse_dev(const SvtB200LrPlane* planes, int n_planes, int64_t* const d_sse[3], int bit_depth, void* stream);
 
 /* ------------------------------------------------------------------------------------------ */
-/* K13 + T2 open-loop ME for a whole picture  (reference: pic_analysis_process.c:130-160,      */
-/*      2138-2190; motion_estimation.c:781-2390; me_process.c:97-291)                          */
+/* K13 HME pyramid + plane padding (pic_analysis_process.c:130-160, 2138-2190) and the T2     */
+/*      open-loop ME driver of a picture (motion_estimation.c:781-3076; me_process.c:97-291)  */
 /* ------------------------------------------------------------------------------------------ */
 /* T1: downsample_2d (aom_dsp_rtcd.h:841). */
 SVT_B200_API void svt_b200_downsample_2d(uint8_t* input_samples, uint32_t input_stride, uint32_t input_area_width,
@@ -728,21 +728,6 @@ typedef struct SvtB200MePicture {
     int32_t reserved[2];
 } SvtB200MePicture;
 
-/* Per-reference search geometry, i.e. the MeContext values the reference derives before searching:
- * hme_l0_sa_* = output of get_hme_l0_search_area (motion_estimation.c:1800-1866) for this reference,
- * hme_l1/l2_sa_* = me_ctx->hme_l1_sa / hme_l2_sa, me_sa_* = MIN(sa_min * scaled_distance, sa_max)
- * (motion_estimation.c:1296-1304). */
-typedef struct SvtB200MeParams {
-    int32_t hme_l0_sa_w, hme_l0_sa_h;
-    int32_t hme_l1_sa_w, hme_l1_sa_h;
-    int32_t hme_l2_sa_w, hme_l2_sa_h;
-    int32_t me_sa_w, me_sa_h;
-    int32_t hme_sub_sad;        /* hme_search_method == SUB_SAD_SEARCH */
-    int32_t me_sub_sad;         /* me_search_method  == SUB_SAD_SEARCH */
-    int32_t check_zero_centre;  /* me_ctx->is_ref: run check_00_center before the full-pel search */
-    int32_t reserved;
-} SvtB200MeParams;
-
 /* replicate the w x h interior at (org_x, org_y) of an 8-bit device plane into its padding
  * (svt_aom_generate_padding / svt_extend_frame) */
 SVT_B200_API int svt_b200_extend_plane_dev(uint8_t* d_buf, int stride, int w, int h, int org_x, int org_y, void* stream);
@@ -757,12 +742,6 @@ typedef struct SvtB200PlaneExtent {
 SVT_B200_API int svt_b200_extend_planes_dev(const SvtB200PlaneExtent* planes, int n_planes, void* stream);
 /* fills the 1/4 and 1/16 planes (interior + replicated padding) from the full plane */
 SVT_B200_API int svt_b200_build_hme_pyramid_dev(const SvtB200MePicture* pic, void* stream);
-/* cur / refs / params are HOST structs holding device plane pointers.  Outputs (device):
- * d_best_sad, d_best_mv: [n_refs][n_b64][85]; d_hme_centre: [n_refs][n_b64][2] (x, y);
- * d_hme_sad: [n_refs][n_b64]. */
-SVT_B200_API int svt_b200_me_picture_dev(const SvtB200MePicture* cur, const SvtB200MePicture* refs,
-                                         const SvtB200MeParams* params, int n_refs, uint32_t* d_best_sad,
-                                         uint32_t* d_best_mv, int16_t* d_hme_centre, uint64_t* d_hme_sad, void* stream);
 
 /* ---- T2, the complete driver: svt_aom_motion_estimation_b64 (motion_estimation.c:3076) for every 64x64 block of a picture ----
  * zz-SAD reference pruning (init_zz_sad :2391), pre-HME (prehme_b64 :1722), HME level 0/1/2 with the early exits and the

@@ -211,152 +211,7 @@ int ref_set_tier(int avx2) {
     return 1;
 }
 
-/* ---- open-loop ME for one picture ---------------------------------------------------------------
- * restates hme_level_0/1/2 (motion_estimation.c:820-1113), set_final_seach_centre_sb (:2182-2390),
- * check_00_center (:1139-1210), integer_search_b64 (:1249-1520), open_loop_me_fullpel_search_sblock
- * (:781-817) for the controls the H100 T2 path honours (see DESIGN.md). */
-#include "ref_me_b64.h" /* the complete driver (ref_me_b64.c) */
-
-static void hme_clip(int16_t org, int16_t* origin, int16_t* sa, int16_t pad, int16_t pic, int round8) {
-    if ((int16_t)(org + *origin) < -pad) {
-        *origin = (int16_t)(-pad - org);
-        *sa     = (int16_t)(*sa - (-pad - (org + *origin)));
-    }
-    if ((int16_t)(org + *origin) > (int16_t)(pic - 1)) *origin = (int16_t)(*origin - ((org + *origin) - (pic - 1)));
-    if ((int16_t)(org + *origin + *sa) > pic) {
-        int16_t v = (int16_t)(*sa - ((org + *origin + *sa) - pic));
-        *sa = v > 1 ? v : 1;
-    }
-    if (round8) *sa = (*sa < 8) ? *sa : (int16_t)(*sa & ~7);
-}
-static int z16(int y16, int x16) { return 4 * (2 * (y16 >> 1) + (x16 >> 1)) + 2 * (y16 & 1) + (x16 & 1); }
-
-static void fullpel_b64(const uint8_t* src, uint32_t ss, const uint8_t* ref, uint32_t rs, int sa_w, int sa_h, int org_x, int org_y, int sub,
-                        uint32_t* best_sad, uint32_t* best_mv) {
-    uint32_t e16[16][8], e8[64][8], e32[4][8], s16[16], s8[64], s32[4];
-    for (int i = 0; i < 85; i++) { best_sad[i] = 128 * 128 * 255; best_mv[i] = 0; }
-    uint32_t *b64 = best_sad, *b32 = best_sad + 1, *b16 = best_sad + 5, *b8 = best_sad + 21;
-    uint32_t *m64 = best_mv, *m32 = best_mv + 1, *m16 = best_mv + 5, *m8 = best_mv + 21;
-    const int w8 = sa_w - (sa_w & 7);
-    for (int y = 0; y < sa_h; y++) {
-        for (int x = 0; x < w8; x += 8) {
-            const uint32_t mv = ((uint32_t)((org_y + y) & 0xffff) << 16) | (uint32_t)((org_x + x) & 0xffff);
-            svt_ext_all_sad_calculation_8x8_16x16((uint8_t*)src, ss, (uint8_t*)ref + (size_t)y * rs + x, rs, mv, b8, b16, m8, m16, e16, e8, sub);
-            svt_ext_eight_sad_calculation_32x32_64x64(e16, b32, b64, m32, m64, mv, e32);
-        }
-        for (int x = w8; x < sa_w; x++) {
-            const uint32_t mv = ((uint32_t)((org_y + y) & 0xffff) << 16) | (uint32_t)((org_x + x) & 0xffff);
-            for (int blk = 0; blk < 16; blk++) {
-                const int y16 = blk >> 2, x16 = blk & 3, i16 = z16(y16, x16);
-                svt_ext_sad_calculation_8x8_16x16((uint8_t*)src + 16 * y16 * ss + 16 * x16, ss,
-                                                  (uint8_t*)ref + (size_t)(y + 16 * y16) * rs + x + 16 * x16, rs, b8 + 4 * i16, b16 + i16,
-                                                  m8 + 4 * i16, m16 + i16, mv, &s16[i16], &s8[4 * i16], sub);
-            }
-            svt_ext_sad_calculation_32x32_64x64(s16, b32, b64, m32, m64, mv, s32);
-        }
-    }
-}
-
-typedef struct { const SvtB200MePicture* cur; const SvtB200MePicture* refs; const SvtB200MeParams* prm; int n_refs; uint32_t* best_sad; uint32_t* best_mv; int16_t* hme_centre; uint64_t* hme_sad; } MeCtx;
-static void ref_me_picture_body(void* vctx, int i) {
-    const MeCtx* c = (const MeCtx*)vctx;
-    const SvtB200MePicture* cur = c->cur;
-    const SvtB200MePicture* refs = c->refs;
-    const SvtB200MeParams* prm = c->prm;
-    uint32_t* best_sad = c->best_sad;
-    uint32_t* best_mv = c->best_mv;
-    int16_t* hme_centre = c->hme_centre;
-    uint64_t* hme_sad = c->hme_sad;
-    const int W = cur->width[2], H = cur->height[2], b64_w = (W + 63) >> 6, b64_h = (H + 63) >> 6, nb = b64_w * b64_h;
-    {
-        const int r = i / nb, b = i % nb, bx = b % b64_w, by = b / b64_w;
-        const SvtB200MePicture* rp = &refs[r];
-        const SvtB200MeParams*  p  = &prm[r];
-        const int sub = p->hme_sub_sad ? 1 : 0;
-        int16_t  px[4] = {0, 0, 0, 0}, py[4] = {0, 0, 0, 0};
-        uint64_t ls[4] = {0, 0, 0, 0};
-        for (int level = 0; level < 3; level++) {
-            const int sh = 2 - level;
-            const int16_t org_x = (int16_t)((bx * 64) >> sh), org_y = (int16_t)((by * 64) >> sh);
-            const int blk_w = (W - bx * 64 < 64 ? W - bx * 64 : 64) >> sh, blk_h = (H - by * 64 < 64 ? H - by * 64 : 64) >> sh;
-            int16_t nx[4], ny[4];
-            for (int reg = 0; reg < 4; reg++) {
-                const int sr_w = reg & 1, sr_h = reg >> 1;
-                int16_t sa_w, sa_h, ox, oy, pw, ph;
-                if (level == 0) {
-                    sa_w = (int16_t)((p->hme_l0_sa_w + 7) & ~7); sa_h = (int16_t)p->hme_l0_sa_h;
-                    ox = (int16_t)(-(int16_t)((sa_w * 2) >> 1) + sa_w * sr_w); oy = (int16_t)(-(int16_t)((sa_h * 2) >> 1) + sa_h * sr_h);
-                    pw = (int16_t)(rp->org_x[0] - 1); ph = (int16_t)(rp->org_y[0] - 1);
-                } else if (level == 1) {
-                    sa_w = (int16_t)((p->hme_l1_sa_w + 7) & ~7); sa_h = (int16_t)p->hme_l1_sa_h;
-                    ox = (int16_t)(-(sa_w >> 1) + (px[reg] >> 1)); oy = (int16_t)(-(sa_h >> 1) + (py[reg] >> 1));
-                    pw = (int16_t)(rp->org_x[1] - 1); ph = (int16_t)(rp->org_y[1] - 1);
-                } else {
-                    sa_w = (int16_t)((p->hme_l2_sa_w + 7) & ~7); sa_h = (int16_t)p->hme_l2_sa_h;
-                    ox = (int16_t)(-(sa_w >> 1) + px[reg]); oy = (int16_t)(-(sa_h >> 1) + py[reg]);
-                    pw = ph = 63;
-                }
-                hme_clip(org_x, &ox, &sa_w, pw, (int16_t)rp->width[level], 1);
-                hme_clip(org_y, &oy, &sa_h, ph, (int16_t)rp->height[level], 0);
-                const uint8_t* s = cur->plane[level] + (size_t)(cur->org_y[level] + org_y) * cur->stride[level] + cur->org_x[level] + org_x;
-                const uint8_t* q = rp->plane[level] + (size_t)(rp->org_y[level] + org_y + oy) * rp->stride[level] + rp->org_x[level] + org_x + ox;
-                uint64_t bs = 0;
-                int16_t  x = 0, y = 0;
-                svt_sad_loop_kernel((uint8_t*)s, (uint32_t)(cur->stride[level] << sub), (uint8_t*)q, (uint32_t)(rp->stride[level] << sub),
-                                    (uint32_t)(blk_h >> sub), (uint32_t)blk_w, &bs, &x, &y, (uint32_t)rp->stride[level], 0, sa_w, sa_h);
-                if (sub) bs *= 2;
-                const int mul = level == 0 ? 4 : (level == 1 ? 2 : 1);
-                nx[reg] = (int16_t)((int16_t)(x + ox) * mul);
-                ny[reg] = (int16_t)((int16_t)(y + oy) * mul);
-                ls[reg] = bs;
-            }
-            memcpy(px, nx, sizeof(px));
-            memcpy(py, ny, sizeof(py));
-        }
-        int16_t  cx = px[0], cy = py[0];
-        uint64_t cs = ls[0];
-        for (int reg = 1; reg < 4; reg++)
-            if (ls[reg] < cs) { cs = ls[reg]; cx = px[reg]; cy = py[reg]; }
-        hme_centre[2 * i] = cx;
-        hme_centre[2 * i + 1] = cy;
-        hme_sad[i] = cs;
-        const int16_t org_x = (int16_t)(bx * 64), org_y = (int16_t)(by * 64);
-        const int blk_w = W - org_x < 64 ? W - org_x : 64, blk_h = H - org_y < 64 ? H - org_y : 64;
-        const uint8_t* src = cur->plane[2] + (size_t)(cur->org_y[2] + org_y) * cur->stride[2] + cur->org_x[2] + org_x;
-        int16_t sx = cx, sy = cy;
-        if (p->check_zero_centre && (sx || sy)) {
-            const int16_t RW = (int16_t)rp->width[2], RH = (int16_t)rp->height[2];
-            if ((int16_t)(org_x + sx) < -63) sx = (int16_t)(-63 - org_x);
-            if ((int16_t)(org_x + sx) > RW - 1) sx = (int16_t)(sx - ((org_x + sx) - (RW - 1)));
-            if ((int16_t)(org_y + sy) < -63) sy = (int16_t)(-63 - org_y);
-            if ((int16_t)(org_y + sy) > RH - 1) sy = (int16_t)(sy - ((org_y + sy) - (RH - 1)));
-            const uint8_t* r0 = rp->plane[2] + (size_t)(rp->org_y[2] + org_y) * rp->stride[2] + rp->org_x[2] + org_x;
-            uint32_t z  = svt_nxm_sad_kernel(src, (uint32_t)cur->stride[2] << 1, r0, (uint32_t)rp->stride[2] << 1, (uint32_t)blk_h >> 1, (uint32_t)blk_w) << 1;
-            uint32_t hs = svt_nxm_sad_kernel(src, (uint32_t)cur->stride[2] << 1, r0 + (ptrdiff_t)sy * rp->stride[2] + sx, (uint32_t)rp->stride[2] << 1,
-                                             (uint32_t)blk_h >> 1, (uint32_t)blk_w) << 1;
-            if (z <= hs) sx = sy = 0;
-        }
-        int16_t sa_w = (int16_t)(((p->me_sa_w > 1 ? p->me_sa_w : 1) + 7) & ~7), sa_h = (int16_t)(p->me_sa_h > 3 ? p->me_sa_h : 3);
-        int16_t ox = (int16_t)(sx - (sa_w >> 1)), oy = (int16_t)(sy - (sa_h >> 1));
-        if ((int16_t)(org_x + ox) < -63) ox = (int16_t)(-63 - org_x);
-        if ((int16_t)(org_x + ox) > W - 1) ox = (int16_t)(ox - ((org_x + ox) - (W - 1)));
-        if ((int16_t)(org_x + ox + sa_w) > W) { int v = sa_w - ((org_x + ox + sa_w) - W); sa_w = (int16_t)(v > 1 ? v : 1); }
-        sa_w = sa_w < 8 ? sa_w : (int16_t)(sa_w & ~7);
-        if ((int16_t)(org_y + oy) < -63) oy = (int16_t)(-63 - org_y);
-        if ((int16_t)(org_y + oy) > H - 1) oy = (int16_t)(oy - ((org_y + oy) - (H - 1)));
-        if ((int16_t)(org_y + oy + sa_h) > H) { int v = sa_h - ((org_y + oy + sa_h) - H); sa_h = (int16_t)(v > 1 ? v : 1); }
-        const uint8_t* q = rp->plane[2] + (ptrdiff_t)(rp->org_y[2] + org_y + oy) * rp->stride[2] + rp->org_x[2] + org_x + ox;
-        fullpel_b64(src, (uint32_t)cur->stride[2], q, (uint32_t)rp->stride[2], sa_w, sa_h, ox, oy, p->me_sub_sad ? 1 : 0, best_sad + (size_t)i * 85,
-                    best_mv + (size_t)i * 85);
-        }
-}
-void ref_me_picture(const SvtB200MePicture* cur, const SvtB200MePicture* refs, const SvtB200MeParams* prm, int n_refs, uint32_t* best_sad,
-                    uint32_t* best_mv, int16_t* hme_centre, uint64_t* hme_sad) {
-    MeCtx c = {cur, refs, prm, n_refs, best_sad, best_mv, hme_centre, hme_sad};
-    const int W = cur->width[2], H = cur->height[2], b64_w = (W + 63) >> 6, b64_h = (H + 63) >> 6, nb = b64_w * b64_h;
-    par_for(n_refs * nb, 4, ref_me_picture_body, &c);
-}
-
+#include "ref_me_b64.h" /* open-loop ME of a picture through the reference's own driver (ref_me_b64.c) */
 
 /* ---- transform / quantize / inverse over a block list ---------------------------------------------
  * the trio of svt_aom_estimate_transform -> svt_aom_quantize_inv_quantize -> inverse (SURVEY 3.4),

@@ -22,8 +22,7 @@ def load_pkg_module(name):
 
 
 layout = load_pkg_module("layout")
-ME_CONTROL_FIELDS, MeControls, MePicture, MeParams, CdefFrame = \
-    layout.ME_CONTROL_FIELDS, layout.MeControls, layout.MePicture, layout.MeParams, layout.CdefFrame
+ME_CONTROL_FIELDS, MeControls, MePicture, CdefFrame = layout.ME_CONTROL_FIELDS, layout.MeControls, layout.MePicture, layout.CdefFrame
 
 
 def pad_np(buf, pad, w, h):
@@ -34,7 +33,8 @@ def pad_np(buf, pad, w, h):
 
 def build_pyramid_np(full, width, height, shapes):
     """numpy restatement of svt_aom_downsample_2d_c + svt_aom_generate_padding
-    (pic_analysis_process.c:130-160, 2138-2190), checked against the reference in tests."""
+    (pic_analysis_process.c:130-160, 2138-2190).  tests/test_me_pyramid.py checks it against the device pyramid
+    (test_build_hme_pyramid_dev), whose downsampling it checks against svt_aom_downsample_2d_c (test_downsample_2d_t1)."""
     planes = [None, None, None]
     th, stride, pad, w, h = shapes[2]
     buf = np.zeros((th, stride), np.uint8)

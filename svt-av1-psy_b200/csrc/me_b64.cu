@@ -26,7 +26,6 @@
 
 #include "common.cuh"
 #include "sad_small.cuh"
-#include "me_hme.cuh"
 #include "../../include/svt_b200.h"
 
 namespace b200 {
@@ -119,14 +118,79 @@ __device__ __forceinline__ uint32_t warp_probe_sads(const uint8_t* src, int ss, 
     return __reduce_add_sync(0xffffffffu, (uint32_t)(d0 * d0) + (uint32_t)(d1 * d1)) / 64u;
 }
 
-// integer_search_b64's clipping of the search window (same arithmetic as the HME levels, against the ALIGNED picture size)
-__device__ __forceinline__ void clip_window(int16_t org, int16_t& o, int16_t& sa, int16_t pad, int16_t pic, bool round8) {
-    const int16_t no = ((int16_t)(org + o) < -pad) ? (int16_t)(-pad - org) : o;
-    sa = ((int16_t)(org + no) < -pad) ? (int16_t)(sa - (-pad - (org + no))) : sa;  // (sic) evaluated with the corrected origin
-    o  = no;
-    o  = ((int16_t)(org + o) > (int16_t)(pic - 1)) ? (int16_t)(o - ((org + o) - (pic - 1))) : o;
-    sa = ((int16_t)(org + o + sa) > pic) ? (int16_t)max(1, sa - ((org + o + sa) - pic)) : sa;
+// One axis of a search window clipped to the reference picture and `pad` pixels of its padding: origin `origin` relative to the
+// block at `org`, size `sa`.  motion_estimation.c writes this clamp out in hme_level_0/1/2 (:848-880, the statement order kept
+// here), prehme_core (:1585-1605) and integer_search_b64 (:1445-1469); the latter two re-test the left edge with the corrected
+// origin before the width step.  Both forms leave sa unchanged there (org + origin == -pad after the correction), and the
+// clamped width (pic - org - origin <= pic + pad) fits int16, so this one function serves all of them.
+__device__ __forceinline__ void clip_search_area(int16_t org, int16_t& origin, int16_t& sa, int16_t pad, int16_t pic, bool round8) {
+    if ((int16_t)(org + origin) < -pad) {
+        origin = (int16_t)(-pad - org);
+        sa     = (int16_t)(sa - (-pad - (org + origin)));  // (sic) evaluates to sa: origin was just moved
+    }
+    if ((int16_t)(org + origin) > (int16_t)(pic - 1)) origin = (int16_t)(origin - ((org + origin) - (pic - 1)));
+    if ((int16_t)(org + origin + sa) > pic) {
+        const int16_t v = (int16_t)(sa - ((org + origin + sa) - pic));
+        sa = v > 1 ? v : (int16_t)1;
+    }
     if (round8) sa = (sa < 8) ? sa : (int16_t)(sa & ~0x07);
+}
+
+// One HME search of region (sr_w, sr_h) of block (bx, by) at `level` (0: 1/16 picture, 1: 1/4, 2: full) over the level's search
+// area (sa_w, sa_h), centred on the previous level's result (prev_x, prev_y; unused at level 0): hme_level_0/1/2 of
+// motion_estimation.c:820-1113 restated as "fill in the search item" + "scale the result back" (hme_finish_one).
+// (origin_x, origin_y): the clipped window origin, which hme_finish_one adds back.
+__device__ __forceinline__ void hme_make_item(const SvtB200MePicture& cur, const SvtB200MePicture& rp, int level, int sa_w_in, int sa_h_in, bool sub_sad,
+                                              int sr_w, int sr_h, int bx, int by, int16_t prev_x, int16_t prev_y,
+                                              SvtB200SadSearchItem& it_out, int16_t& origin_x, int16_t& origin_y) {
+    const int shift = 2 - level;
+    const int full_x = bx * 64, full_y = by * 64;
+    const int blk_w = min(64, cur.width[2] - full_x) >> shift, blk_h = min(64, cur.height[2] - full_y) >> shift;
+    const int16_t org_x = (int16_t)(full_x >> shift), org_y = (int16_t)(full_y >> shift);
+    int16_t sa_w = (int16_t)((sa_w_in + 7) & ~0x07), sa_h = (int16_t)sa_h_in, ox, oy, pad_w, pad_h;
+    if (level == 0) {
+        ox   = (int16_t)(-(int16_t)((sa_w * 2) >> 1) + sa_w * sr_w);
+        oy   = (int16_t)(-(int16_t)((sa_h * 2) >> 1) + sa_h * sr_h);
+        pad_w = (int16_t)(rp.org_x[0] - 1);
+        pad_h = (int16_t)(rp.org_y[0] - 1);
+    } else if (level == 1) {
+        ox   = (int16_t)(-(sa_w >> 1) + (prev_x >> 1));
+        oy   = (int16_t)(-(sa_h >> 1) + (prev_y >> 1));
+        pad_w = (int16_t)(rp.org_x[1] - 1);
+        pad_h = (int16_t)(rp.org_y[1] - 1);
+    } else {
+        ox   = (int16_t)(-(sa_w >> 1) + prev_x);
+        oy   = (int16_t)(-(sa_h >> 1) + prev_y);
+        pad_w = pad_h = 63;
+    }
+    clip_search_area(org_x, ox, sa_w, pad_w, (int16_t)rp.width[level], true);
+    clip_search_area(org_y, oy, sa_h, pad_h, (int16_t)rp.height[level], false);
+    const int sub = sub_sad ? 1 : 0;
+    SvtB200SadSearchItem it;
+    it.src_off    = (uint64_t)(uintptr_t)(cur.plane[level] + (size_t)(cur.org_y[level] + org_y) * cur.stride[level] + cur.org_x[level] + org_x);
+    it.ref_off    = (uint64_t)(uintptr_t)(rp.plane[level] + (size_t)(rp.org_y[level] + org_y + oy) * rp.stride[level] + rp.org_x[level] + org_x + ox);
+    it.src_stride = (uint32_t)(cur.stride[level] << sub);
+    it.ref_stride = (uint32_t)(rp.stride[level] << sub);
+    it.ref_step   = (uint32_t)rp.stride[level];
+    it.block_w    = (uint16_t)blk_w;
+    it.block_h    = (uint16_t)(blk_h >> sub);
+    it.sa_w       = sa_w;
+    it.sa_h       = sa_h;
+    it.skip_search_line = 0;
+    it.reserved   = 0;
+    it_out   = it;
+    origin_x = ox;
+    origin_y = oy;
+}
+
+__device__ __forceinline__ void hme_finish_one(const SvtB200SadSearchResult& q, int16_t origin_x, int16_t origin_y, bool sub_sad, int level,
+                                               int16_t& out_x, int16_t& out_y, uint64_t& out_sad) {
+    const int mul = level == 0 ? 4 : (level == 1 ? 2 : 1);
+    uint64_t  sad = q.best_sad;
+    if (sub_sad) sad *= 2;
+    out_sad = sad;
+    out_x   = (int16_t)((int16_t)(q.x + origin_x) * mul);
+    out_y   = (int16_t)((int16_t)(q.y + origin_y) * mul);
 }
 
 template <int PAR>  // references whose HME runs concurrently in a CTA (4 warps each)
@@ -245,8 +309,8 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
                     int16_t       sa_h = (int16_t)(uint16_t)min(c.prehme_sa[sr][1] * f, c.prehme_sa[sr][3]);
                     const int16_t ox16 = (int16_t)(org_x >> 2), oy16 = (int16_t)(org_y >> 2);
                     int16_t       ox = (int16_t)-(int16_t)(sa_w >> 1), oy = (int16_t)-(int16_t)(sa_h >> 1);
-                    hme_clip(ox16, ox, sa_w, (int16_t)(rp.org_x[0] - 1), (int16_t)rp.width[0], false);
-                    hme_clip(oy16, oy, sa_h, (int16_t)(rp.org_y[0] - 1), (int16_t)rp.height[0], false);
+                    clip_search_area(ox16, ox, sa_w, (int16_t)(rp.org_x[0] - 1), (int16_t)rp.width[0], false);
+                    clip_search_area(oy16, oy, sa_h, (int16_t)(rp.org_y[0] - 1), (int16_t)rp.height[0], false);
                     const int sub = c.hme_sub_sad ? 1 : 0;
                     SvtB200SadSearchItem it;
                     it.src_off = it.ref_off = 0;
@@ -314,11 +378,6 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
             const bool on = (warp >> 2) < par && p < n_pairs;
             const int  l = on ? pair_l(p) : 0, r = on ? pair_r(p) : 0;
             const SvtB200MePicture& rp = tab.ref[l][r];
-            SvtB200MeParams prm;
-            prm.hme_l1_sa_w = c.hme_l1_w; prm.hme_l1_sa_h = c.hme_l1_h; prm.hme_l2_sa_w = c.hme_l2_w; prm.hme_l2_sa_h = c.hme_l2_h;
-            prm.hme_sub_sad = c.hme_sub_sad; prm.me_sub_sad = c.me_sub_sad; prm.check_zero_centre = 0; prm.reserved = 0;
-            prm.me_sa_w = prm.me_sa_h = 0;
-            prm.hme_l0_sa_w = prm.hme_l0_sa_h = 0;
             const bool zz_exit = on && c.me_early_exit_th && s.zz[l][r] < ((uint32_t)c.me_early_exit_th >> 2);
             // ---- level 0 (hme_level0_b64)
             if (c.enable_l0) {
@@ -352,16 +411,14 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
                         sa_w = (int16_t)min(((sa_w * f) + 15) & ~0x0F, ((max_w / 2) + 15) & ~0x0F);
                         int16_t sa_h = (int16_t)(min_h / 2);
                         sa_h = (int16_t)min(sa_h * f, max_h / 2);
-                        prm.hme_l0_sa_w = sa_w;
-                        prm.hme_l0_sa_h = sa_h;
                         SvtB200SadSearchItem it;
-                        HmeSide              sd;
-                        hme_make_item(cur, rp, prm, 0, reg & 1, reg >> 1, bx, by, 0, 0, it, sd);
+                        int16_t              o_x, o_y;
+                        hme_make_item(cur, rp, 0, sa_w, sa_h, c.hme_sub_sad, reg & 1, reg >> 1, bx, by, 0, 0, it, o_x, o_y);
                         const SvtB200SadSearchResult q =
                             sad_key_to_result(sad_search_warp((const uint8_t*)(uintptr_t)it.src_off, (const uint8_t*)(uintptr_t)it.ref_off, it, lane));
                         int16_t  x, y;
                         uint64_t sad;
-                        hme_finish_one(q, sd, prm, 0, x, y, sad);
+                        hme_finish_one(q, o_x, o_y, c.hme_sub_sad, 0, x, y, sad);
                         if (lane == 0) { s.lx[0][l][r][reg] = x; s.ly[0][l][r][reg] = y; s.lsad[0][l][r][reg] = sad; }
                     }
                 }
@@ -396,13 +453,13 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
                     if (lane == 0) { s.lx[1][l][r][reg] = s.lx[0][l][r][reg]; s.ly[1][l][r][reg] = s.ly[0][l][r][reg]; s.lsad[1][l][r][reg] = s.lsad[0][l][r][reg]; }
                 } else {
                     SvtB200SadSearchItem it;
-                    HmeSide              sd;
-                    hme_make_item(cur, rp, prm, 1, reg & 1, reg >> 1, bx, by, s.lx[0][l][r][reg], s.ly[0][l][r][reg], it, sd);
+                    int16_t              o_x, o_y;
+                    hme_make_item(cur, rp, 1, c.hme_l1_w, c.hme_l1_h, c.hme_sub_sad, reg & 1, reg >> 1, bx, by, s.lx[0][l][r][reg], s.ly[0][l][r][reg], it, o_x, o_y);
                     const SvtB200SadSearchResult q =
                         sad_key_to_result(sad_search_warp((const uint8_t*)(uintptr_t)it.src_off, (const uint8_t*)(uintptr_t)it.ref_off, it, lane));
                     int16_t  x, y;
                     uint64_t sad;
-                    hme_finish_one(q, sd, prm, 1, x, y, sad);
+                    hme_finish_one(q, o_x, o_y, c.hme_sub_sad, 1, x, y, sad);
                     if (lane == 0) { s.lx[1][l][r][reg] = x; s.ly[1][l][r][reg] = y; s.lsad[1][l][r][reg] = sad; }
                 }
                 __syncwarp();
@@ -413,13 +470,13 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
                     if (lane == 0) { s.lx[2][l][r][reg] = s.lx[1][l][r][reg]; s.ly[2][l][r][reg] = s.ly[1][l][r][reg]; s.lsad[2][l][r][reg] = s.lsad[1][l][r][reg]; }
                 } else {
                     SvtB200SadSearchItem it;
-                    HmeSide              sd;
-                    hme_make_item(cur, rp, prm, 2, reg & 1, reg >> 1, bx, by, s.lx[1][l][r][reg], s.ly[1][l][r][reg], it, sd);
+                    int16_t              o_x, o_y;
+                    hme_make_item(cur, rp, 2, c.hme_l2_w, c.hme_l2_h, c.hme_sub_sad, reg & 1, reg >> 1, bx, by, s.lx[1][l][r][reg], s.ly[1][l][r][reg], it, o_x, o_y);
                     const SvtB200SadSearchResult q =
                         sad_key_to_result(sad_search_warp((const uint8_t*)(uintptr_t)it.src_off, (const uint8_t*)(uintptr_t)it.ref_off, it, lane));
                     int16_t  x, y;
                     uint64_t sad;
-                    hme_finish_one(q, sd, prm, 2, x, y, sad);
+                    hme_finish_one(q, o_x, o_y, c.hme_sub_sad, 2, x, y, sad);
                     if (lane == 0) { s.lx[2][l][r][reg] = x; s.ly[2][l][r][reg] = y; s.lsad[2][l][r][reg] = sad; }
                 }
                 __syncwarp();
@@ -541,8 +598,8 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
             it.seed_y = sy;
         }
         int16_t ox = (int16_t)(sx - (sa_w >> 1)), oy = (int16_t)(sy - (sa_h >> 1));
-        clip_window(org_x, ox, sa_w, 63, (int16_t)aw, true);
-        clip_window(org_y, oy, sa_h, 63, (int16_t)ah, false);
+        clip_search_area(org_x, ox, sa_w, 63, (int16_t)aw, true);  // against the 8-aligned picture size (:3093-3100)
+        clip_search_area(org_y, oy, sa_h, 63, (int16_t)ah, false);
         it.ref_off = (uint64_t)(uintptr_t)(r0 + (ptrdiff_t)oy * rp.stride[2] + ox);
         it.sa_w = sa_w;
         it.sa_h = sa_h;

@@ -202,7 +202,7 @@ struct FpTma {
     int32_t n_b64;                                // items are ordered (reference, b64)
 };
 
-// TMA = true (open-loop ME of a picture, svt_b200_me_picture_dev): source block and search-window boxes arrive by TMA,
+// TMA = true (open-loop ME of a picture, svt_b200_me_b64_picture_dev): source block and search-window boxes arrive by TMA,
 // double-buffered -- the box of the next (item, chunk) is in flight while the current one is searched.
 // TMA = false (svt_b200_fullpel_search_batch_dev on caller planes of unknown extent): staged by the threads.
 template <bool TMA>
@@ -393,7 +393,7 @@ static bool make_plane_map(CUtensorMap* m, const uint8_t* base, int pitch, int r
     return r == CUDA_SUCCESS;
 }
 
-// full-pel search of a picture's (reference, b64) items through TMA; false = geometry not expressible (caller falls back)
+// full-pel search of a picture's (reference, b64) items through TMA; false = geometry not expressible (the caller fails)
 bool launch_fullpel_tma(const SvtB200MePicture* cur, const SvtB200MePicture* refs, int n_refs, int n_b64, const SvtB200FullpelItem* d_items,
                         int n_items, uint32_t* d_best_sad, uint32_t* d_best_mv, cudaStream_t st, const uint32_t* d_seed_sad) {
     if (n_refs > kFpTmaRefs) return false;

@@ -1,4 +1,4 @@
-// sad_small.cuh -- warp-level full search over a SMALL search area (shared by sad.cu and me_picture.cu).
+// sad_small.cuh -- warp-level full search over a SMALL search area (shared by sad.cu and me_b64.cu).
 //
 // Small search areas (the 8x3 / 16x4 HME and ME refinements: a few dozen positions, blocks up to
 // 64x64): the work is a few hundred VABSDIFF4 per lane, so staging through shared memory and CTA

@@ -416,8 +416,6 @@ lib.svt_b200_downsample_2d.argtypes = [vp, ct.c_uint32, ct.c_uint32, ct.c_uint32
 lib.svt_b200_downsample_2d.restype = None
 lib.svt_b200_build_hme_pyramid_dev.argtypes = [ct.POINTER(MePicture), vp]
 lib.svt_b200_build_hme_pyramid_dev.restype = ct.c_int
-lib.svt_b200_me_picture_dev.argtypes = [ct.POINTER(MePicture), ct.POINTER(MePicture), ct.POINTER(MeParams), ct.c_int, vp, vp, vp, vp, vp]
-lib.svt_b200_me_picture_dev.restype = ct.c_int
 lib.svt_b200_me_b64_num_pus.argtypes = [ct.POINTER(MeControls)]
 lib.svt_b200_me_b64_num_pus.restype = ct.c_int
 lib.svt_b200_me_b64_picture_dev.argtypes = [ct.POINTER(MePicture), ct.POINTER(MePicture), ct.POINTER(MeControls), ct.POINTER(MeB64Results), vp]

@@ -187,11 +187,6 @@ class MePicture(ct.Structure):
                [("reserved", ct.c_int32 * 2)]
 
 
-class MeParams(ct.Structure):
-    _fields_ = _same(ct.c_int32, "hme_l0_sa_w", "hme_l0_sa_h", "hme_l1_sa_w", "hme_l1_sa_h", "hme_l2_sa_w", "hme_l2_sa_h", "me_sa_w",
-                     "me_sa_h", "hme_sub_sad", "me_sub_sad", "check_zero_centre", "reserved")
-
-
 class PlaneExtent(ct.Structure):
     _fields_ = [("buf", ct.c_void_p)] + _same(ct.c_int32, "stride", "w", "h", "org_x", "org_y", "pixel_bytes")
 

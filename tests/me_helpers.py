@@ -1,12 +1,11 @@
 """Reference-driven full-pel search: replays open_loop_me_fullpel_search_sblock
 (motion_estimation.c:781-817) in Python on top of the UNMODIFIED reference kernels
 (svt_ext_all_sad_calculation_8x8_16x16_c, svt_ext_eight_sad_calculation_32x32_64x64_c and the
-1-point variants), so that the 85-PU results are produced by the reference's own update code."""
+1-point variants), so that the 85-PU results are produced by the reference's own update code; and the synthetic
+pictures the picture-level ME checks search."""
 import ctypes as ct
 
 import numpy as np
-
-from oracle import support as sp
 
 MAX_SAD = 128 * 128 * 255
 
@@ -66,147 +65,25 @@ def hadamard_call(lib, name, src, stride, n):
     return out
 
 
-# ---- whole-picture open-loop ME, driven on the reference kernels ------------------------------------
-def i16(v):
-    v &= 0xffff
-    return v - 0x10000 if v & 0x8000 else v
+def sequence(r, w, h, n, pan=(3, 1), noise=4.0, still_rect=None):
+    """n pictures of a panning synthetic scene (optionally with a static rectangle: early-exit / stationary paths)"""
+    yy, xx = np.mgrid[0:h + 160, 0:w + 160]
+    base = (np.sin(xx / 13.0) * 45 + np.cos(yy / 9.0) * 35 + ((xx // 20 + yy // 28) % 2) * 70 + ((xx // 7) % 3) * 9 + 100)
+    out = []
+    for t in range(n):
+        ox, oy = 80 + pan[0] * (t - n // 2), 80 + pan[1] * (t - n // 2)
+        img = base[oy:oy + h, ox:ox + w] + r.normal(0, noise, (h, w))
+        if still_rect is not None:
+            x0, y0, x1, y1 = still_rect
+            img[y0:y1, x0:x1] = base[80 + y0:80 + y1, 80 + x0:80 + x1] + r.normal(0, 0.6, (y1 - y0, x1 - x0))
+        out.append(np.clip(img, 0, 255).astype(np.uint8))
+    return out
 
 
-def build_pyramid_np(full, width, height, shapes):
-    """numpy restatement of svt_aom_downsample_2d_c + svt_aom_generate_padding (checked against the
-    reference function in test_oracle_pins)."""
-    planes = [None, None, None]
-    th, stride, pad, w, h = shapes[2]
-    buf = np.zeros((th, stride), np.uint8)
-    buf[pad:pad + h, pad:pad + w] = full
-    planes[2] = pad_np(buf, pad, w, h)
-    src = full.astype(np.uint32)
-    for lvl in (1, 0):
-        th, stride, pad, w, h = shapes[lvl]
-        d = ((src[0::2, 0::2] + src[0::2, 1::2] + src[1::2, 0::2] + src[1::2, 1::2] + 2) >> 2)[:h, :w]
-        buf = np.zeros((th, stride), np.uint8)
-        buf[pad:pad + h, pad:pad + w] = d
-        planes[lvl] = pad_np(buf, pad, w, h)
-        src = d.astype(np.uint32)
-    return planes
-
-
-def pad_np(buf, pad, w, h):
-    inner = buf[pad:pad + h, pad:pad + w]
-    buf[:, :] = np.pad(inner, ((pad, buf.shape[0] - pad - h), (pad, buf.shape[1] - pad - w)), mode="edge")
-    return buf
-
-
-def hme_clip(org, origin, sa, pad, pic, round8):
-    if i16(org + origin) < -pad:
-        origin = i16(-pad - org)
-        sa = i16(sa - (-pad - (org + origin)))
-    if i16(org + origin) > pic - 1:
-        origin = i16(origin - ((org + origin) - (pic - 1)))
-    if i16(org + origin + sa) > pic:
-        sa = max(1, i16(sa - ((org + origin + sa) - pic)))
-    if round8:
-        sa = sa if sa < 8 else sa & ~7
-    return origin, sa
-
-
-def ref_me_picture(refc, cur, refs, shapes, width, height, params, sad_fn="svt_sad_loop_kernel_c"):
-    """cur/refs: lists of 3 padded numpy planes.  Returns (best_sad, best_mv, hme_centre, hme_sad)."""
-    from helpers import sad_loop_call
-    b64_w, b64_h = (width + 63) // 64, (height + 63) // 64
-    nb = b64_w * b64_h
-    R = len(refs)
-    out_sad = np.zeros((R, nb, 85), np.uint32); out_mv = np.zeros((R, nb, 85), np.uint32)
-    out_c = np.zeros((R, nb, 2), np.int16); out_hs = np.zeros((R, nb), np.uint64)
-    curf = [p.reshape(-1) for p in cur]
-    for r in range(R):
-        p = params[r]
-        reff = [q.reshape(-1) for q in refs[r]]
-        sub = 1 if p["hme_sub_sad"] else 0
-        for b in range(nb):
-            bx, by = b % b64_w, b // b64_w
-            prev = [(0, 0)] * 4
-            lsad = [0] * 4
-            for level in range(3):
-                th, stride, pad, w, h = shapes[level]
-                sh = 2 - level
-                org_x, org_y = (bx * 64) >> sh, (by * 64) >> sh
-                blk_w, blk_h = min(64, width - bx * 64) >> sh, min(64, height - by * 64) >> sh
-                nxt = []
-                for reg in range(4):
-                    sr_w, sr_h = reg & 1, reg >> 1
-                    if level == 0:
-                        sa_w = (p["hme_l0_sa_w"] + 7) & ~7; sa_h = p["hme_l0_sa_h"]
-                        ox = i16(-((sa_w * 2) >> 1) + sa_w * sr_w); oy = i16(-((sa_h * 2) >> 1) + sa_h * sr_h)
-                        pw = ph = pad - 1
-                    elif level == 1:
-                        sa_w = (p["hme_l1_sa_w"] + 7) & ~7; sa_h = p["hme_l1_sa_h"]
-                        ox = i16(-(sa_w >> 1) + (prev[reg][0] >> 1)); oy = i16(-(sa_h >> 1) + (prev[reg][1] >> 1))
-                        pw = ph = pad - 1
-                    else:
-                        sa_w = (p["hme_l2_sa_w"] + 7) & ~7; sa_h = p["hme_l2_sa_h"]
-                        ox = i16(-(sa_w >> 1) + prev[reg][0]); oy = i16(-(sa_h >> 1) + prev[reg][1])
-                        pw = ph = 63
-                    ox, sa_w = hme_clip(org_x, ox, sa_w, pw, w, True)
-                    oy, sa_h = hme_clip(org_y, oy, sa_h, ph, h, False)
-                    s_off = (pad + org_y) * stride + pad + org_x
-                    r_off = (pad + org_y + oy) * stride + pad + org_x + ox
-                    best, x, y = sad_loop_call(refc, sad_fn, curf[level], s_off, stride << sub, reff[level], r_off, stride << sub,
-                                               blk_h >> sub, blk_w, stride, 0, sa_w, sa_h)
-                    if sub:
-                        best *= 2
-                    mul = 4 if level == 0 else (2 if level == 1 else 1)
-                    nxt.append((i16(i16(x + ox) * mul), i16(i16(y + oy) * mul)))
-                    lsad[reg] = best
-                prev = nxt
-            cx, cy, cs = prev[0][0], prev[0][1], lsad[0]
-            for reg in range(1, 4):
-                if lsad[reg] < cs:
-                    cs, cx, cy = lsad[reg], prev[reg][0], prev[reg][1]
-            out_c[r, b] = (cx, cy); out_hs[r, b] = cs
-            th, stride, pad, w, h = shapes[2]
-            org_x, org_y = bx * 64, by * 64
-            blk_w, blk_h = min(64, width - org_x), min(64, height - org_y)
-            sx, sy = cx, cy
-            s_off = (pad + org_y) * stride + pad + org_x
-            if p["check_zero_centre"] and (sx != 0 or sy != 0):
-                if i16(org_x + sx) < -63: sx = i16(-63 - org_x)
-                if i16(org_x + sx) > w - 1: sx = i16(sx - ((org_x + sx) - (w - 1)))
-                if i16(org_y + sy) < -63: sy = i16(-63 - org_y)
-                if i16(org_y + sy) > h - 1: sy = i16(sy - ((org_y + sy) - (h - 1)))
-                f = refc.svt_nxm_sad_kernel_helper_c; f.restype = ct.c_uint32
-                z = f(P(curf[2], s_off), ct.c_uint32(stride * 2), P(reff[2], s_off), ct.c_uint32(stride * 2), blk_h >> 1, blk_w) << 1
-                hs = f(P(curf[2], s_off), ct.c_uint32(stride * 2), P(reff[2], s_off + sy * stride + sx), ct.c_uint32(stride * 2), blk_h >> 1,
-                       blk_w) << 1
-                if z <= hs:
-                    sx = sy = 0
-            sa_w = (max(1, p["me_sa_w"]) + 7) & ~7; sa_h = max(3, p["me_sa_h"])
-            ox, oy = i16(sx - (sa_w >> 1)), i16(sy - (sa_h >> 1))
-            if i16(org_x + ox) < -63: ox = i16(-63 - org_x)
-            if i16(org_x + ox) > width - 1: ox = i16(ox - ((org_x + ox) - (width - 1)))
-            if i16(org_x + ox + sa_w) > width: sa_w = max(1, sa_w - ((org_x + ox + sa_w) - width))
-            sa_w = sa_w if sa_w < 8 else sa_w & ~7
-            if i16(org_y + oy) < -63: oy = i16(-63 - org_y)
-            if i16(org_y + oy) > height - 1: oy = i16(oy - ((org_y + oy) - (height - 1)))
-            if i16(org_y + oy + sa_h) > height: sa_h = max(1, sa_h - ((org_y + oy + sa_h) - height))
-            r_off = (pad + org_y + oy) * stride + pad + org_x + ox
-            sad, mv = ref_fullpel(refc, curf[2], s_off, stride, reff[2], r_off, stride, sa_w, sa_h, ox, oy, p["me_sub_sad"])
-            out_sad[r, b] = sad; out_mv[r, b] = mv
-    return out_sad, out_mv, out_c, out_hs
-
-
-def ref_me_picture_c(refc, cur, refs, shapes, width, height, params):
-    """the pthread C driver in oracle/ref_driver.c (reference kernels through the dispatch pointers)"""
-    R = len(refs)
-    nb = ((width + 63) // 64) * ((height + 63) // 64)
-    sad = np.zeros((R, nb, 85), np.uint32); mv = np.zeros((R, nb, 85), np.uint32)
-    c = np.zeros((R, nb, 2), np.int16); hs = np.zeros((R, nb), np.uint64)
-    cd = sp.ref_pic_desc(cur, shapes)
-    rd = (sp.MePicture * R)(*[sp.ref_pic_desc(r, shapes) for r in refs])
-    pr = (sp.MeParams * R)()
-    for i, p in enumerate(params):
-        for k, v in p.items():
-            setattr(pr[i], k, v)
-    refc.ref_me_picture.restype = None
-    refc.ref_me_picture(ct.byref(cd), rd, pr, R, P(sad), P(mv), P(c), P(hs))
-    return sad, mv, c, hs
+def case_pictures(r, w, h, n_ref, dist, content):
+    """(current picture, reference pictures of list 0 then list 1) of a test_me_b64.CASES entry: nine pictures of `sequence`,
+    the current one in the middle, each reference as many pictures away as its distance says (at most four)"""
+    seq = sequence(r, w, h, 2 * 4 + 1, **content)
+    mid = len(seq) // 2
+    pick = lambda d: seq[int(np.clip(mid + np.sign(d) * min(abs(d), 4), 0, len(seq) - 1))]  # noqa: E731
+    return seq[mid], [pick(dist[0][i]) for i in range(n_ref[0])] + [pick(dist[1][i]) for i in range(n_ref[1])]

@@ -16,21 +16,6 @@ from oracle import support as sp
 pytestmark = pytest.mark.gpu
 
 
-def _sequence(r, w, h, n, pan=(3, 1), noise=4.0, still_rect=None):
-    """n pictures of a panning synthetic scene (optionally with a static rectangle: early-exit / stationary paths)"""
-    yy, xx = np.mgrid[0:h + 160, 0:w + 160]
-    base = (np.sin(xx / 13.0) * 45 + np.cos(yy / 9.0) * 35 + ((xx // 20 + yy // 28) % 2) * 70 + ((xx // 7) % 3) * 9 + 100)
-    out = []
-    for t in range(n):
-        ox, oy = 80 + pan[0] * (t - n // 2), 80 + pan[1] * (t - n // 2)
-        img = base[oy:oy + h, ox:ox + w] + r.normal(0, noise, (h, w))
-        if still_rect is not None:
-            x0, y0, x1, y1 = still_rect
-            img[y0:y1, x0:x1] = base[80 + y0:80 + y1, 80 + x0:80 + x1] + r.normal(0, 0.6, (y1 - y0, x1 - x0))
-        out.append(np.clip(img, 0, 255).astype(np.uint8))
-    return out
-
-
 CASES = [
     # name, W, H, preset, n_ref, poc distances, temporal layer, is_ref, extra cfg, content
     ("m8_nonbase_2p2", 448, 272, 8, (2, 2), ((-1, -3, 0, 0), (1, 3, 0, 0)), 3, 0, {}, dict(pan=(3, 1), still_rect=(128, 64, 320, 192))),
@@ -51,13 +36,10 @@ def test_me_b64_matches_reference_driver(b200, refc, case):
     r = rng(500 + len(name))
     shapes = b200.me_plane_shapes(W, H)
     n_pic = n_ref[0] + n_ref[1] + 1
-    seq = _sequence(r, W, H, 2 * 4 + 1, **content)
-    mid = len(seq) // 2
     # reference pictures: list 0 looks back, list 1 forward (or back again on a base-layer picture); the step follows the distance
-    pick = lambda d: seq[int(np.clip(mid + np.sign(d) * min(abs(d), 4), 0, len(seq) - 1))]  # noqa: E731
-    fulls = [pick(dist[0][i]) for i in range(n_ref[0])] + [pick(dist[1][i]) for i in range(n_ref[1])]
-    cur_np = mh.build_pyramid_np(seq[mid], W, H, shapes)
-    refs_np = [mh.build_pyramid_np(f, W, H, shapes) for f in fulls]
+    cur_full, fulls = mh.case_pictures(r, W, H, n_ref, dist, content)
+    cur_np = sp.build_pyramid_np(cur_full, W, H, shapes)
+    refs_np = [sp.build_pyramid_np(f, W, H, shapes) for f in fulls]
     cfg = sp.me_b64_cfg(preset=preset, n_ref=n_ref, poc_dist=dist, temporal_layer_index=tl, is_ref=is_ref, **extra)
     ctrl, want = sp.ref_me_b64_picture(refc, cur_np, refs_np, shapes, cfg)
     cd = ctrl.as_dict()

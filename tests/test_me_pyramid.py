@@ -1,6 +1,7 @@
 """GPU parity: Hadamard/SATD (picture_operators_c.c:188-330), the SAD pyramid T1 kernels
-(motion_estimation.c:98-427; fixtures modelled on test/SadTest.cc:731-1306) and the T2 85-PU
-full-pel search against the reference kernels driven in the reference's own loop order."""
+(motion_estimation.c:98-427; fixtures modelled on test/SadTest.cc:731-1306), the T2 85-PU
+full-pel search against the reference kernels driven in the reference's own loop order, and the
+HME pyramid (downsample_2d + padding, pic_analysis_process.c:130-160, 2138-2190)."""
 import ctypes as ct
 
 import numpy as np
@@ -8,6 +9,7 @@ import pytest
 
 import me_helpers as mh
 from helpers import rng
+from oracle import support as sp
 
 pytestmark = pytest.mark.gpu
 
@@ -111,6 +113,38 @@ def test_fullpel_search_batch(b200, oracle):
         want = mh.ref_fullpel(oracle.ref, *args) if oracle.ref is not None else mh.port_fullpel(oracle.port, *args)
         assert np.array_equal(sad[i], want[0]), i
         assert np.array_equal(mv[i], want[1]), i
+
+
+def test_downsample_2d_t1(b200, refc):
+    r = rng(120)
+    f = refc.svt_aom_downsample_2d_c; f.restype = None
+    for (w, h, step) in [(64, 48, 2), (130, 70, 2), (64, 64, 4)]:
+        src = r.integers(0, 256, (h, w + 6)).astype(np.uint8)
+        ow, oh = w // step, h // step
+        a = np.zeros((oh, ow + 3), np.uint8); b = a.copy()
+        f(mh.P(src), w + 6, w, h, mh.P(a), ow + 3, step)
+        b200.lib.svt_b200_downsample_2d(mh.P(src), w + 6, w, h, mh.P(b), ow + 3, step)
+        assert np.array_equal(a, b)
+
+
+def test_build_hme_pyramid_dev(b200):
+    """T2: the padded 1/4 and 1/16 planes (interior and padding) built on the device from the full plane == oracle.support's
+    build_pyramid_np, at 320x200 (5 x 4 blocks of 64x64, the last row 8 high)"""
+    import torch
+    W, H = 320, 200
+    shapes = b200.me_plane_shapes(W, H)
+    for full in mh.sequence(rng(121), W, H, 2):
+        want = sp.build_pyramid_np(full, W, H, shapes)
+        planes = [torch.zeros((s[0], s[1]), dtype=torch.uint8, device="cuda") for s in shapes]
+        pad = shapes[2][2]
+        planes[2][pad:pad + H, pad:pad + W] = torch.from_numpy(full).cuda()
+        # full-resolution padding is the caller's job (svt_aom_generate_padding on the input picture)
+        planes[2].copy_(torch.from_numpy(sp.pad_np(planes[2].cpu().numpy(), pad, W, H)))
+        d = b200.me_picture_desc(planes, W, H)
+        assert b200.lib.svt_b200_build_hme_pyramid_dev(ct.byref(d), None) == 0
+        torch.cuda.synchronize()
+        for lvl in range(3):
+            assert np.array_equal(planes[lvl].cpu().numpy(), want[lvl]), lvl
 
 
 def test_hadamard_path_fwht_and_cul_level(b200, refc):

@@ -254,32 +254,33 @@ def test_port_selfguided_and_projection_match_reference(oracle, refc):
                 assert np.array_equal(da, db.astype(np.uint16)), (bd, w, h, kind)
 
 
-# ---- picture-level reference drivers (oracle/ref_driver.c) ---------------------------------------
-def test_ref_driver_me_matches_numpy_driver_and_avx2_tier(oracle, refc):
-    from test_me_picture import _content
-    r = rng(130)
-    W, H = 320, 200
-    ME_PAD = (16, 32, 72)
-    shapes = []
-    for lvl in range(3):
-        w, h, pad = W >> (2 - lvl), H >> (2 - lvl), ME_PAD[lvl]
-        shapes.append((h + 2 * pad, (w + 2 * pad + 15) & ~15, pad, w, h))
-    cur = mh.build_pyramid_np(_content(r, W, H, (0, 0)), W, H, shapes)
-    refs = [mh.build_pyramid_np(_content(r, W, H, (5, -3)), W, H, shapes), mh.build_pyramid_np(_content(r, W, H, (-19, 9)), W, H, shapes)]
-    params = [dict(hme_l0_sa_w=16, hme_l0_sa_h=8, hme_l1_sa_w=8, hme_l1_sa_h=3, hme_l2_sa_w=8, hme_l2_sa_h=3, me_sa_w=8, me_sa_h=3,
-                   hme_sub_sad=0, me_sub_sad=0, check_zero_centre=1),
-              dict(hme_l0_sa_w=32, hme_l0_sa_h=12, hme_l1_sa_w=8, hme_l1_sa_h=3, hme_l2_sa_w=8, hme_l2_sa_h=3, me_sa_w=16, me_sa_h=5,
-                   hme_sub_sad=1, me_sub_sad=1, check_zero_centre=0)]
-    refc.ref_set_tier(0)
-    a = mh.ref_me_picture(refc, cur, refs, shapes, W, H, params)
-    b = mh.ref_me_picture_c(refc, cur, refs, shapes, W, H, params)
-    for x, y in zip(a, b):
-        assert np.array_equal(x, y)
-    if refc.ref_set_tier(1) == 1:  # the intrinsics-only AVX2 tier must agree with the C tier
-        c = mh.ref_me_picture_c(refc, cur, refs, shapes, W, H, params)
-        for x, y in zip(b, c):
-            assert np.array_equal(x, y)
-    refc.ref_set_tier(0)
+# ---- picture-level reference drivers (oracle/ref_driver.c, oracle/ref_me_b64.c) --------------------------
+@pytest.mark.parametrize("case", ["m8_nonbase_2p2", "m2_mvsa_zero_centre"])
+def test_ref_me_b64_avx2_tier_matches_c_tier(refc, case):
+    """the reference arm of the benchmark runs the reference's own open-loop ME driver (oracle/ref_me_b64.c) at the
+    intrinsics-only AVX2 tier: on the pictures of a test_me_b64 case, every output equals the C tier's"""
+    from oracle import support as sp
+    from test_me_b64 import CASES
+    name, W, H, preset, n_ref, dist, tl, is_ref, extra, content = next(c for c in CASES if c[0] == case)
+    shapes = sp.layout.me_plane_shapes(W, H)
+    cur_full, fulls = mh.case_pictures(rng(500 + len(name)), W, H, n_ref, dist, content)
+    cur = sp.build_pyramid_np(cur_full, W, H, shapes)
+    refs = [sp.build_pyramid_np(f, W, H, shapes) for f in fulls]
+    cfg = sp.me_b64_cfg(preset=preset, n_ref=n_ref, poc_dist=dist, temporal_layer_index=tl, is_ref=is_ref, **extra)
+    if refc.ref_set_tier(1) != 1:
+        pytest.skip("the host has no AVX2")
+    try:
+        outs = []
+        for tier in (0, 1):
+            assert refc.ref_set_tier(tier) == tier
+            outs.append(sp.ref_me_b64_picture(refc, cur, refs, shapes, cfg))
+    finally:
+        refc.ref_set_tier(0)
+    (ctrl_c, want), (ctrl_avx2, got) = outs
+    assert ctrl_c.as_dict() == ctrl_avx2.as_dict()
+    assert sorted(want) == sorted(got)
+    for k in want:
+        assert np.array_equal(want[k], got[k]), k
 
 
 def test_committed_golden_fixtures_are_what_the_reference_computes(oracle, refc):
