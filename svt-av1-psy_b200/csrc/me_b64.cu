@@ -15,9 +15,12 @@
 //   compute_distortion              :2964
 //   perform_gm_detection            :2842
 //
-// Launches:  (A) me_b64_hme_kernel<PAR>  one CTA per 64x64 block, 4 * PAR warps.  The references are walked in the reference's
-//                order, PAR at a time (1, or 2 from six references up: chosen on the previous target GPU, not re-measured on H100); inside the HME stages a warp is one
-//                (reference, search region) pair, in the per-reference stages (zz SAD, pre-HME, window derivation) one reference.
+// Launches:  (A) me_b64_hme_kernel  one CTA of 8 warps per 64x64 block, at most 64 registers a thread (four CTAs fill an SM's
+//                register file).  zz SADs and the search-window derivation: one warp per reference.  Pre-HME (list 0, then
+//                list 1) and HME levels 0, 1, 2: each stage is a list of independent warp jobs built in shared memory by warp 0
+//                (lane = one (reference, band) or (reference, search region) slot, taking the reference's early-exit decisions),
+//                one job loop over all warps, a barrier, and warp 0 turning the jobs' keys into the stage's results.  A
+//                pre-HME band is cut into row slices of about equal work, each a job, merged by the minimum key.
 //                Decisions that couple references (pruning, carried-over centres) are taken by one thread between barriers.
 //                Writes one full-pel item per (reference, block) + the 85 SADs of the variance probe ("seed").
 //            (B) fullpel_search_kernel<TMA> (me_pyramid.cu) over the items, best arrays seeded with the probe.
@@ -55,6 +58,9 @@ struct B64State {
     int16_t  sc_x[2][kDepth], sc_y[2][kDepth];
     uint64_t hme_sad[2][kDepth];
     uint32_t divisor[2][kDepth];
+    // the block: position, and size in the 8-aligned picture.  Read from here where it is needed, so that no register holds it
+    // through the searches between.
+    int16_t  org_x, org_y, blk_w, blk_h;
 };
 
 __device__ __forceinline__ int scaled_distance(int dist) { return (dist * 5) / 8 + ((dist % 8) == 0 ? 0 : 1); }  // svt_aom_get_scaled_picture_distance
@@ -193,26 +199,53 @@ __device__ __forceinline__ void hme_finish_one(const SvtB200SadSearchResult& q, 
     out_y   = (int16_t)((int16_t)(q.y + origin_y) * mul);
 }
 
-template <int PAR>  // references whose HME runs concurrently in a CTA (4 warps each)
-__global__ void __launch_bounds__(128 * PAR, PAR == 1 ? 4 : 3)
+constexpr int kHmeThreads = 256;  // 8 warps: the CTA of one 64x64 block
+constexpr int kSlots      = 32;   // results of one stage: (pair, search region) at the HME levels, (reference, band) in pre-HME
+constexpr int kMaxSlices  = 8;    // row slices of one pre-HME search
+constexpr int kSliceTiles = 32;   // 8-position tiles a slice is cut to hold (the order of the short band's whole search)
+constexpr int kMaxJobs    = 8 * kMaxSlices;
+
+// The searches of one stage.  A job searches window rows [y0, y0 + h) of its slot's search and merges its best key
+// (sad << 32 | y << 16 | x, y counted from the window's first row) into key[slot] by the minimum: the raster-order first
+// minimum of the whole window, whatever the cut.
+struct JobList {
+    SvtB200SadSearchItem item[kSlots];            // the slot's whole search
+    SvtB200SadSearchItem job[kMaxJobs];           // a slice of it; searched in place (a copy in registers spills at 64)
+    unsigned long long   key[kSlots];
+    int16_t              ox[kSlots], oy[kSlots];  // clipped window origin of the slot's search
+    uint32_t             slot_y0[kMaxJobs];       // slot | y0 << 8
+    uint8_t              on[kSlots];              // the slot searches
+    int                  n;
+};
+
+// Stages that search: pre-HME of list 0, then of list 1 (whose early exit reads list 0's results), HME level 0 in two rounds
+// (the second holds the references whose level-0 area reads the result of list 0 / reference 0 in the low-delay
+// "reduce_hme_l0_sr" mode, and is empty otherwise), level 1, level 2.
+enum { kPh0, kPh1, kL0a, kL0b, kL1, kL2, kStages };
+
+__global__ void __launch_bounds__(kHmeThreads, 4)
 me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, SvtB200FullpelItem* __restrict__ items,
                   uint32_t* __restrict__ seed_sad, uint8_t* __restrict__ st_do_ref /*[n_b64][8]*/, int16_t* __restrict__ out_centre,
                   uint32_t* __restrict__ out_zz) {
     __shared__ B64State s;
+    __shared__ JobList  jb;
     const SvtB200MeControls& c = tab.c;
     const SvtB200MePicture&  cur = tab.cur;
-    const int b = blockIdx.x, bx = b % b64_w, by = b / b64_w, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
-    const int W = cur.width[2], H = cur.height[2];
-    const int16_t org_x = (int16_t)(bx * 64), org_y = (int16_t)(by * 64);
+    const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, n_warps = blockDim.x >> 5;
     // me_ctx->b64_width / b64_height come from the 8-aligned picture size (:3093-3100)
-    const int aw = (W + 7) & ~7, ah = (H + 7) & ~7;
-    const int blk_w = min(64, aw - org_x), blk_h = min(64, ah - org_y);
+    const int aw = (cur.width[2] + 7) & ~7, ah = (cur.height[2] + 7) & ~7;
     const int n_pairs = c.n_ref[0] + (c.n_list > 1 ? c.n_ref[1] : 0);
     auto pair_l = [&](int p) { return p < c.n_ref[0] ? 0 : 1; };
     auto pair_r = [&](int p) { return p < c.n_ref[0] ? p : p - c.n_ref[0]; };
-    const uint8_t* src_full = cur.plane[2] + (size_t)(cur.org_y[2] + org_y) * cur.stride[2] + cur.org_x[2] + org_x;
+    auto block_src = [&]() { return cur.plane[2] + (size_t)(cur.org_y[2] + s.org_y) * cur.stride[2] + cur.org_x[2] + s.org_x; };
 
     // ---- init_me_hme_data ------------------------------------------------------------------------------------------
+    if (threadIdx.x == 0) {
+        s.org_x = (int16_t)((b % b64_w) * 64);
+        s.org_y = (int16_t)((b / b64_w) * 64);
+        s.blk_w = (int16_t)min(64, aw - s.org_x);
+        s.blk_h = (int16_t)min(64, ah - s.org_y);
+    }
     for (int i = threadIdx.x; i < 2 * kDepth; i += blockDim.x) {
         const int l = i / kDepth, r = i % kDepth;
         s.zz[l][r] = kMaxU32;
@@ -233,11 +266,12 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
     }
     __syncthreads();
 
-    // ---- init_zz_sad -------------------------------------------------------------------------------------------------
+    // ---- init_zz_sad: warp = reference -----------------------------------------------------------------------------------
     if (c.me_early_exit_th || c.me_safe_limit_zz_th) {
-        for (int p = warp; p < n_pairs; p += n_warps) {
-            const int l = pair_l(p), r = pair_r(p);
-            if (!searched(c, l)) continue;
+        if (warp < n_pairs && searched(c, pair_l(warp))) {
+            const int      p = warp, l = pair_l(p), r = pair_r(p);
+            const int16_t  org_x = s.org_x, org_y = s.org_y, blk_w = s.blk_w, blk_h = s.blk_h;
+            const uint8_t* src_full = block_src();
             const SvtB200MePicture& rp = tab.ref[l][r];
             const uint8_t* r0 = rp.plane[2] + (size_t)(rp.org_y[2] + org_y) * rp.stride[2] + rp.org_x[2] + org_x;
             uint32_t z = warp_sad_every_other_row(src_full, cur.stride[2], r0, rp.stride[2], blk_w, blk_h, lane) << 1;
@@ -267,165 +301,212 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
         __syncthreads();
     }
 
-    // ---- prehme_b64 ----------------------------------------------------------------------------------------------------
-    if (c.prehme_enable) {
-        const int max_r = max(c.n_ref[0], c.n_list > 1 ? c.n_ref[1] : 0);
-        // unit = (reference index, search region); the warp walks list 0 then list 1 of its unit: list 1 may copy list 0's result
-        for (int u = warp; u < max_r * 2; u += n_warps) {
-            const int r = u >> 1, sr = u & 1;
-            for (int l = 0; l < c.n_list; l++) {
-                if (r >= c.n_ref[l]) continue;
-                if (!searched(c, l)) {  // base layer: list 1 mirrors list 0 (valid / performed flags are not touched)
-                    if (lane == 0) {
-                        s.ph_x[1][r][sr] = (int16_t)-s.ph_x[0][r][sr];
-                        s.ph_y[1][r][sr] = (int16_t)-s.ph_y[0][r][sr];
-                        s.ph_sad[1][r][sr] = s.ph_sad[0][r][sr];
+    // ---- prehme_b64 and hme_level0/1/2_b64 ------------------------------------------------------------------------------
+    // Each stage: warp 0 takes the decisions of the stage's slots (lane = slot) and lists the searches; every warp takes jobs
+    // from the list; warp 0 turns the merged keys into the stage's results.
+    const bool coupled = c.sr_enable && c.sr_distance_based_hme_resizing && c.reduce_hme_l0_sr_th_min && c.reduce_hme_l0_sr_th_max;
+    const int  split   = coupled ? 1 : n_pairs;  // level-0 rounds: pairs [0, split), then [split, n_pairs)
+    // which branch of hme_level0_b64 a reference takes: 0 zz exit, 1 previous-stage exit, 2 pruned, 3 search, 4 not searched (base layer, list 1)
+    auto l0_kind = [&](int li, int ri) {
+        const int sr_i = s.ph_sad[li][ri][0] <= s.ph_sad[li][ri][1] ? 0 : 1;
+        if (c.me_early_exit_th && s.zz[li][ri] < ((uint32_t)c.me_early_exit_th >> 2)) return 0;
+        if (c.prev_me_stage_based_exit_th && s.ph_done[li][ri][sr_i] && s.ph_sad[li][ri][sr_i] < ((uint32_t)c.prev_me_stage_based_exit_th >> 4)) return 1;
+        if (!s.do_ref[li][ri]) return 2;
+        return searched(c, li) ? 3 : 4;
+    };
+    for (int stage = 0; stage < kStages; stage++) {
+        const bool ph = stage <= kPh1;
+        const int  lv = stage <= kL0b ? 0 : stage - kL1 + 1;
+        const int  p_lo = stage == kL0b ? split : 0, p_hi = stage == kL0a ? split : n_pairs;
+        bool run;
+        if (ph) run = c.prehme_enable && stage < c.n_list;
+        else if (lv == 0) run = c.enable_hme && c.enable_l0 && p_lo < p_hi;
+        else run = c.enable_hme && (lv == 1 ? c.enable_l1 : c.enable_l2);
+        if (run) {
+            if (warp == 0) {
+                bool mine = false;  // this lane's slot searches
+                SvtB200SadSearchItem& it = jb.item[lane];
+                int nsl = 0, h = 0, total_h = 0;  // slices, window rows per slice, of the whole window
+                if (ph) {
+                    // check_prehme_early_exit, then prehme_core; lane = (reference, band)
+                    const int l = stage, r = lane >> 1, sr = lane & 1;
+                    if (lane < 2 * c.n_ref[l]) {
+                        if (!searched(c, l)) {  // base layer: list 1 mirrors list 0 (valid / performed flags are not touched)
+                            s.ph_x[1][r][sr] = (int16_t)-s.ph_x[0][r][sr];
+                            s.ph_y[1][r][sr] = (int16_t)-s.ph_y[0][r][sr];
+                            s.ph_sad[1][r][sr] = s.ph_sad[0][r][sr];
+                        } else if (c.me_early_exit_th && s.zz[l][r] < (uint32_t)c.me_early_exit_th) {
+                            s.ph_x[l][r][sr] = s.ph_y[l][r][sr] = 0;
+                            s.ph_sad[l][r][sr] = 0;
+                            s.ph_valid[l][r][sr] = 1;
+                        } else if (c.prehme_l1_early_exit && l == 1 && s.ph_valid[0][r][sr] &&
+                                   (s.ph_sad[0][r][sr] < 32 * 32 || (abs((int)s.ph_x[0][r][sr]) < 16 && abs((int)s.ph_y[0][r][sr]) < 16))) {
+                            s.ph_x[1][r][sr] = (int16_t)-s.ph_x[0][r][sr];
+                            s.ph_y[1][r][sr] = (int16_t)-s.ph_y[0][r][sr];
+                            s.ph_sad[1][r][sr] = s.ph_sad[0][r][sr];
+                            s.ph_valid[1][r][sr] = 1;
+                        } else if (!s.do_ref[l][r]) {
+                            s.ph_x[l][r][sr] = s.ph_y[l][r][sr] = 0;
+                            s.ph_sad[l][r][sr] = kMaxU32;
+                        } else {
+                            const SvtB200MePicture& rp = tab.ref[l][r];
+                            const int     f = scaled_distance(c.dist[l][r]);
+                            int16_t       sa_w = (int16_t)(uint16_t)min(c.prehme_sa[sr][0] * f, c.prehme_sa[sr][2]);
+                            int16_t       sa_h = (int16_t)(uint16_t)min(c.prehme_sa[sr][1] * f, c.prehme_sa[sr][3]);
+                            const int16_t ox16 = (int16_t)(s.org_x >> 2), oy16 = (int16_t)(s.org_y >> 2);
+                            int16_t       ox = (int16_t)-(int16_t)(sa_w >> 1), oy = (int16_t)-(int16_t)(sa_h >> 1);
+                            clip_search_area(ox16, ox, sa_w, (int16_t)(rp.org_x[0] - 1), (int16_t)rp.width[0], false);
+                            clip_search_area(oy16, oy, sa_h, (int16_t)(rp.org_y[0] - 1), (int16_t)rp.height[0], false);
+                            const int sub = c.hme_sub_sad ? 1 : 0;
+                            it.src_off = (uint64_t)(uintptr_t)(cur.plane[0] + (size_t)(cur.org_y[0] + oy16) * cur.stride[0] + cur.org_x[0] + ox16);
+                            it.ref_off = (uint64_t)(uintptr_t)(rp.plane[0] + (ptrdiff_t)(rp.org_y[0] + oy16 + oy) * rp.stride[0] + rp.org_x[0] + ox16 + ox);
+                            it.src_stride = (uint32_t)(cur.stride[0] << sub);
+                            it.ref_stride = (uint32_t)(rp.stride[0] << sub);
+                            it.ref_step   = (uint32_t)rp.stride[0];
+                            it.block_w    = (uint16_t)(s.blk_w >> 2);
+                            it.block_h    = (uint16_t)((s.blk_h >> 2) >> sub);
+                            it.sa_w = sa_w;
+                            it.sa_h = sa_h;
+                            it.skip_search_line = (uint16_t)c.prehme_skip_search_line;
+                            it.reserved = 0;
+                            // the band's rows in slices of about kSliceTiles tiles; a slice starts on an even window row, so that with
+                            // line skipping it evaluates exactly the window's odd rows in its range
+                            const int rows = c.prehme_skip_search_line ? sa_h >> 1 : sa_h;
+                            nsl = min(kMaxSlices, max(1, (((sa_w + 7) >> 3) * rows + kSliceTiles - 1) / kSliceTiles));
+                            h   = max(2, (((sa_h + nsl - 1) / nsl) + 1) & ~1);
+                            nsl = max(1, (sa_h + h - 1) / h);
+                            total_h = sa_h;
+                            jb.ox[lane] = ox;
+                            jb.oy[lane] = oy;
+                            jb.key[lane] = ~0ull;
+                            mine = true;
+                        }
                     }
-                    __syncwarp();
-                    continue;
-                }
-                // check_prehme_early_exit
-                bool done = false;
-                if (c.me_early_exit_th && s.zz[l][r] < (uint32_t)c.me_early_exit_th) {
-                    if (lane == 0) { s.ph_x[l][r][sr] = s.ph_y[l][r][sr] = 0; s.ph_sad[l][r][sr] = 0; s.ph_valid[l][r][sr] = 1; }
-                    done = true;
-                } else if (c.prehme_l1_early_exit && l == 1 && s.ph_valid[0][r][sr] &&
-                           (s.ph_sad[0][r][sr] < 32 * 32 || (abs((int)s.ph_x[0][r][sr]) < 16 && abs((int)s.ph_y[0][r][sr]) < 16))) {
-                    if (lane == 0) {
-                        s.ph_x[1][r][sr] = (int16_t)-s.ph_x[0][r][sr];
-                        s.ph_y[1][r][sr] = (int16_t)-s.ph_y[0][r][sr];
-                        s.ph_sad[1][r][sr] = s.ph_sad[0][r][sr];
-                        s.ph_valid[1][r][sr] = 1;
+                } else {
+                    // lane = (pair, search region)
+                    const int p = lane >> 2, reg = lane & 3;
+                    if (p >= p_lo && p < p_hi) {
+                        const int l = pair_l(p), r = pair_r(p);
+                        int       sa_w = 0, sa_h = 0;
+                        int16_t   prev_x = 0, prev_y = 0;
+                        int16_t&  out_x = s.lx[lv][l][r][reg];
+                        int16_t&  out_y = s.ly[lv][l][r][reg];
+                        uint64_t& out_sad = s.lsad[lv][l][r][reg];
+                        if (lv == 0) {
+                            const int kind = l0_kind(l, r);
+                            const int sr_i = s.ph_sad[l][r][0] <= s.ph_sad[l][r][1] ? 0 : 1;
+                            if (kind == 0) {
+                                out_x = out_y = 0;
+                                out_sad = 0;
+                            } else if (kind == 1) {
+                                out_x = s.ph_x[l][r][sr_i];
+                                out_y = s.ph_y[l][r][sr_i];
+                                out_sad = s.ph_sad[l][r][sr_i];
+                            } else if (kind == 2) {
+                                out_x = out_y = 0;
+                                out_sad = kMaxU32;
+                            } else if (kind == 3) {
+                                // get_hme_l0_search_area
+                                int min_w = c.hme_l0_min_w, min_h = c.hme_l0_min_h, max_w = c.hme_l0_max_w, max_h = c.hme_l0_max_h;
+                                if (c.sr_enable && c.sr_distance_based_hme_resizing) {
+                                    bool is_hor = true, is_ver = true, is_still = false;
+                                    if (c.reduce_hme_l0_sr_th_min && c.reduce_hme_l0_sr_th_max && (l || r)) {
+                                        const int mx = abs((int)s.lx[0][0][0][0]), my = abs((int)s.ly[0][0][0][0]);
+                                        is_ver   = mx < c.reduce_hme_l0_sr_th_min && my > c.reduce_hme_l0_sr_th_max;
+                                        is_hor   = mx > c.reduce_hme_l0_sr_th_max && my < c.reduce_hme_l0_sr_th_min;
+                                        is_still = mx < c.reduce_hme_l0_sr_th_min * 3 && my < c.reduce_hme_l0_sr_th_min * 3;
+                                    }
+                                    int x_off = is_hor ? 1 : 2, y_off = is_ver ? 1 : 2;
+                                    if (c.sr_enable == 2 && is_still) x_off = y_off = 4;
+                                    min_w = (uint16_t)(min_w / (x_off + r)); min_h = (uint16_t)(min_h / (y_off + r));
+                                    max_w = (uint16_t)(max_w / (x_off + r)); max_h = (uint16_t)(max_h / (y_off + r));
+                                }
+                                const int f = scaled_distance(c.dist[l][r]);
+                                int16_t w16 = (int16_t)(min_w / 2);
+                                w16 = (int16_t)min(((w16 * f) + 15) & ~0x0F, ((max_w / 2) + 15) & ~0x0F);
+                                int16_t h16 = (int16_t)(min_h / 2);
+                                h16 = (int16_t)min(h16 * f, max_h / 2);
+                                sa_w = w16;
+                                sa_h = h16;
+                                mine = true;
+                            }
+                        } else if (searched(c, l)) {
+                            const uint32_t prev_th = (uint32_t)c.prev_me_stage_based_exit_th;
+                            if (lv == 1 && c.me_early_exit_th && s.zz[l][r] < ((uint32_t)c.me_early_exit_th >> 2)) {
+                                out_x = out_y = 0;
+                                out_sad = 0;
+                            } else if (lv == 1 && !s.do_ref[l][r]) {
+                                out_x = out_y = 0;
+                                out_sad = kMaxU32;
+                            } else if (prev_th && s.lsad[lv - 1][l][r][reg] < (prev_th >> (lv == 1 ? 5 : 2))) {
+                                out_x = s.lx[lv - 1][l][r][reg];
+                                out_y = s.ly[lv - 1][l][r][reg];
+                                out_sad = s.lsad[lv - 1][l][r][reg];
+                            } else {  // level 2 has no other exit: pruned references are searched as well
+                                sa_w   = lv == 1 ? c.hme_l1_w : c.hme_l2_w;
+                                sa_h   = lv == 1 ? c.hme_l1_h : c.hme_l2_h;
+                                prev_x = s.lx[lv - 1][l][r][reg];
+                                prev_y = s.ly[lv - 1][l][r][reg];
+                                mine   = true;
+                            }
+                        }
+                        if (mine) {
+                            int16_t o_x, o_y;
+                            hme_make_item(cur, tab.ref[l][r], lv, sa_w, sa_h, c.hme_sub_sad, reg & 1, reg >> 1, s.org_x >> 6, s.org_y >> 6, prev_x, prev_y, it, o_x,
+                                          o_y);
+                            jb.ox[lane] = o_x;
+                            jb.oy[lane] = o_y;
+                            jb.key[lane] = ~0ull;
+                            nsl = 1;
+                            h   = total_h = it.sa_h;
+                        }
                     }
-                    done = true;
-                } else if (!s.do_ref[l][r]) {
-                    if (lane == 0) { s.ph_x[l][r][sr] = s.ph_y[l][r][sr] = 0; s.ph_sad[l][r][sr] = kMaxU32; }
-                    done = true;
                 }
-                if (!done) {  // prehme_core
-                    const SvtB200MePicture& rp = tab.ref[l][r];
-                    const int     f = scaled_distance(c.dist[l][r]);
-                    int16_t       sa_w = (int16_t)(uint16_t)min(c.prehme_sa[sr][0] * f, c.prehme_sa[sr][2]);
-                    int16_t       sa_h = (int16_t)(uint16_t)min(c.prehme_sa[sr][1] * f, c.prehme_sa[sr][3]);
-                    const int16_t ox16 = (int16_t)(org_x >> 2), oy16 = (int16_t)(org_y >> 2);
-                    int16_t       ox = (int16_t)-(int16_t)(sa_w >> 1), oy = (int16_t)-(int16_t)(sa_h >> 1);
-                    clip_search_area(ox16, ox, sa_w, (int16_t)(rp.org_x[0] - 1), (int16_t)rp.width[0], false);
-                    clip_search_area(oy16, oy, sa_h, (int16_t)(rp.org_y[0] - 1), (int16_t)rp.height[0], false);
-                    const int sub = c.hme_sub_sad ? 1 : 0;
-                    SvtB200SadSearchItem it;
-                    it.src_off = it.ref_off = 0;
-                    it.src_stride = (uint32_t)(cur.stride[0] << sub);
-                    it.ref_stride = (uint32_t)(rp.stride[0] << sub);
-                    it.ref_step   = (uint32_t)rp.stride[0];
-                    it.block_w    = (uint16_t)(blk_w >> 2);
-                    it.block_h    = (uint16_t)((blk_h >> 2) >> sub);
-                    it.sa_w = sa_w;
-                    it.sa_h = sa_h;
-                    it.skip_search_line = (uint16_t)c.prehme_skip_search_line;
-                    it.reserved = 0;
-                    const uint8_t* sp = cur.plane[0] + (size_t)(cur.org_y[0] + oy16) * cur.stride[0] + cur.org_x[0] + ox16;
-                    const uint8_t* rq = rp.plane[0] + (ptrdiff_t)(rp.org_y[0] + oy16 + oy) * rp.stride[0] + rp.org_x[0] + ox16 + ox;
-                    const SvtB200SadSearchResult q = sad_key_to_result(sad_search_warp(sp, rq, it, lane));
-                    if (lane == 0) {
+                // job list: this lane's slices after those of the lanes below it
+                int end = nsl;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int v = __shfl_up_sync(0xffffffffu, end, o);
+                    if (lane >= o) end += v;
+                }
+                if (lane == 31) jb.n = end;
+                jb.on[lane] = mine;
+                for (int k = 0, j = end - nsl; k < nsl; k++, j++) {
+                    jb.job[j] = it;
+                    jb.job[j].ref_off += (uint64_t)(k * h) * it.ref_step;
+                    jb.job[j].sa_h = (int16_t)min(h, total_h - k * h);
+                    jb.slot_y0[j] = (uint32_t)lane | (uint32_t)(k * h) << 8;
+                }
+            }
+            __syncthreads();
+            for (int j = warp; j < jb.n; j += n_warps) {
+                const unsigned long long k = sad_search_warp<2>((const uint8_t*)(uintptr_t)jb.job[j].src_off, (const uint8_t*)(uintptr_t)jb.job[j].ref_off, jb.job[j], lane);
+                if (lane == 0 && k != ~0ull) atomicMin(&jb.key[jb.slot_y0[j] & 0xff], k + ((unsigned long long)(jb.slot_y0[j] >> 8) << 16));
+            }
+            __syncthreads();
+            if (warp == 0) {
+                if (jb.on[lane]) {
+                    const SvtB200SadSearchResult q = sad_key_to_result(jb.key[lane]);
+                    if (ph) {
+                        const int  l = stage, r = lane >> 1, sr = lane & 1;
                         const bool none = q.x < 0;  // no line evaluated: the reference keeps the MV of an earlier block; (0,0) here (DESIGN 6)
-                        uint64_t sad = q.best_sad;
-                        if (sub) sad *= 2;
+                        uint64_t   sad = q.best_sad;
+                        if (c.hme_sub_sad) sad *= 2;
                         s.ph_sad[l][r][sr] = sad;
-                        s.ph_x[l][r][sr] = (int16_t)((int16_t)((none ? 0 : q.x) + ox) * 4);
-                        s.ph_y[l][r][sr] = (int16_t)((int16_t)((none ? 0 : q.y) + oy) * 4);
+                        s.ph_x[l][r][sr] = (int16_t)((int16_t)((none ? 0 : q.x) + jb.ox[lane]) * 4);
+                        s.ph_y[l][r][sr] = (int16_t)((int16_t)((none ? 0 : q.y) + jb.oy[lane]) * 4);
                         s.ph_valid[l][r][sr] = 1;
                         s.ph_done[l][r][sr] = 1;
+                    } else {
+                        const int p = lane >> 2, reg = lane & 3, l = pair_l(p), r = pair_r(p);
+                        hme_finish_one(q, jb.ox[lane], jb.oy[lane], c.hme_sub_sad, lv, s.lx[lv][l][r][reg], s.ly[lv][l][r][reg], s.lsad[lv][l][r][reg]);
                     }
                 }
-                __syncwarp();
-            }
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            uint32_t best = kMaxU32;
-            for (int p = 0; p < n_pairs; p++) {
-                const int l = pair_l(p), r = pair_r(p);
-                if (!searched(c, l)) continue;
-                best = min(best, (uint32_t)min(s.ph_sad[l][r][0], s.ph_sad[l][r][1]));
-            }
-            if (c.temporal_layer_index > 0 && best < (uint32_t)c.phme_sad_th)
-                for (int p = 0; p < n_pairs; p++) {
-                    const int l = pair_l(p), r = pair_r(p);
-                    if (!s.do_ref[l][r] || r == 0) continue;
-                    const uint32_t ps = (uint32_t)min(s.ph_sad[l][r][0], s.ph_sad[l][r][1]);
-                    if ((uint32_t)((ps - best) * 100u) > (uint32_t)((uint32_t)c.phme_sad_pct * best)) s.do_ref[l][r] = 0;
-                }
-        }
-        __syncthreads();
-    }
-
-    // ---- HME level 0 / 1 / 2: warp = (reference, search region); `par` references at a time, in order ------------------------------
-    // (the only coupling between references inside these stages is the low-delay "reduce_hme_l0_sr" rule, which reads the level-0
-    //  centre of list 0 / reference 0: with it on, the references go one at a time)
-    if (c.enable_hme) {
-        const bool coupled = c.sr_enable && c.sr_distance_based_hme_resizing && c.reduce_hme_l0_sr_th_min && c.reduce_hme_l0_sr_th_max;
-        const int  par = coupled ? 1 : max(1, n_warps >> 2), reg = warp & 3;
-        // which branch of hme_level0_b64 a reference takes: 0 zz exit, 1 previous-stage exit, 2 pruned, 3 search, 4 not searched (base layer, list 1)
-        auto l0_kind = [&](int li, int ri) {
-            const int sr_i = s.ph_sad[li][ri][0] <= s.ph_sad[li][ri][1] ? 0 : 1;
-            if (c.me_early_exit_th && s.zz[li][ri] < ((uint32_t)c.me_early_exit_th >> 2)) return 0;
-            if (c.prev_me_stage_based_exit_th && s.ph_done[li][ri][sr_i] && s.ph_sad[li][ri][sr_i] < ((uint32_t)c.prev_me_stage_based_exit_th >> 4)) return 1;
-            if (!s.do_ref[li][ri]) return 2;
-            return searched(c, li) ? 3 : 4;
-        };
-        for (int p0 = 0; p0 < n_pairs; p0 += par) {
-            const int  p = p0 + (warp >> 2);
-            const bool on = (warp >> 2) < par && p < n_pairs;
-            const int  l = on ? pair_l(p) : 0, r = on ? pair_r(p) : 0;
-            const SvtB200MePicture& rp = tab.ref[l][r];
-            const bool zz_exit = on && c.me_early_exit_th && s.zz[l][r] < ((uint32_t)c.me_early_exit_th >> 2);
-            // ---- level 0 (hme_level0_b64)
-            if (c.enable_l0) {
-                if (on) {
-                    const int kind = l0_kind(l, r);
-                    const int sr_i = s.ph_sad[l][r][0] <= s.ph_sad[l][r][1] ? 0 : 1;
-                    if (kind == 0) {
-                        if (lane == 0) { s.lx[0][l][r][reg] = s.ly[0][l][r][reg] = 0; s.lsad[0][l][r][reg] = 0; }
-                    } else if (kind == 1) {
-                        if (lane == 0) { s.lx[0][l][r][reg] = s.ph_x[l][r][sr_i]; s.ly[0][l][r][reg] = s.ph_y[l][r][sr_i]; s.lsad[0][l][r][reg] = s.ph_sad[l][r][sr_i]; }
-                    } else if (kind == 2) {
-                        if (lane == 0) { s.lx[0][l][r][reg] = s.ly[0][l][r][reg] = 0; s.lsad[0][l][r][reg] = kMaxU32; }
-                    } else if (kind == 3) {
-                        // get_hme_l0_search_area
-                        int min_w = c.hme_l0_min_w, min_h = c.hme_l0_min_h, max_w = c.hme_l0_max_w, max_h = c.hme_l0_max_h;
-                        if (c.sr_enable && c.sr_distance_based_hme_resizing) {
-                            bool is_hor = true, is_ver = true, is_still = false;
-                            if (c.reduce_hme_l0_sr_th_min && c.reduce_hme_l0_sr_th_max && (l || r)) {
-                                const int mx = abs((int)s.lx[0][0][0][0]), my = abs((int)s.ly[0][0][0][0]);
-                                is_ver   = mx < c.reduce_hme_l0_sr_th_min && my > c.reduce_hme_l0_sr_th_max;
-                                is_hor   = mx > c.reduce_hme_l0_sr_th_max && my < c.reduce_hme_l0_sr_th_min;
-                                is_still = mx < c.reduce_hme_l0_sr_th_min * 3 && my < c.reduce_hme_l0_sr_th_min * 3;
-                            }
-                            int x_off = is_hor ? 1 : 2, y_off = is_ver ? 1 : 2;
-                            if (c.sr_enable == 2 && is_still) x_off = y_off = 4;
-                            min_w = (uint16_t)(min_w / (x_off + r)); min_h = (uint16_t)(min_h / (y_off + r));
-                            max_w = (uint16_t)(max_w / (x_off + r)); max_h = (uint16_t)(max_h / (y_off + r));
-                        }
-                        const int f = scaled_distance(c.dist[l][r]);
-                        int16_t sa_w = (int16_t)(min_w / 2);
-                        sa_w = (int16_t)min(((sa_w * f) + 15) & ~0x0F, ((max_w / 2) + 15) & ~0x0F);
-                        int16_t sa_h = (int16_t)(min_h / 2);
-                        sa_h = (int16_t)min(sa_h * f, max_h / 2);
-                        SvtB200SadSearchItem it;
-                        int16_t              o_x, o_y;
-                        hme_make_item(cur, rp, 0, sa_w, sa_h, c.hme_sub_sad, reg & 1, reg >> 1, bx, by, 0, 0, it, o_x, o_y);
-                        const SvtB200SadSearchResult q =
-                            sad_key_to_result(sad_search_warp((const uint8_t*)(uintptr_t)it.src_off, (const uint8_t*)(uintptr_t)it.ref_off, it, lane));
-                        int16_t  x, y;
-                        uint64_t sad;
-                        hme_finish_one(q, o_x, o_y, c.hme_sub_sad, 0, x, y, sad);
-                        if (lane == 0) { s.lx[0][l][r][reg] = x; s.ly[0][l][r][reg] = y; s.lsad[0][l][r][reg] = sad; }
-                    }
-                }
-                __syncthreads();  // the four regions' level-0 results of these references are complete
-                if (c.prehme_enable) {  // replace the worst quadrant of a searched reference by its better pre-HME result
-                    if ((int)threadIdx.x < par && p0 + (int)threadIdx.x < n_pairs) {
-                        const int li = pair_l(p0 + threadIdx.x), ri = pair_r(p0 + threadIdx.x);
+                if (lv == 0 && !ph && c.prehme_enable) {  // replace the worst quadrant of a searched reference by its better pre-HME result
+                    __syncwarp();
+                    const int p = p_lo + lane;
+                    if (p < p_hi) {
+                        const int li = pair_l(p), ri = pair_r(p);
                         if (l0_kind(li, ri) == 3) {
                             const int sr_i = s.ph_sad[li][ri][0] <= s.ph_sad[li][ri][1] ? 0 : 1;
                             uint64_t  mx = 0;
@@ -440,50 +521,29 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
                             }
                         }
                     }
-                    __syncthreads();
                 }
             }
-            // ---- level 1 (hme_level1_b64)
-            if (on && c.enable_l1 && searched(c, l)) {
-                if (zz_exit) {
-                    if (lane == 0) { s.lx[1][l][r][reg] = s.ly[1][l][r][reg] = 0; s.lsad[1][l][r][reg] = 0; }
-                } else if (!s.do_ref[l][r]) {
-                    if (lane == 0) { s.lx[1][l][r][reg] = s.ly[1][l][r][reg] = 0; s.lsad[1][l][r][reg] = kMaxU32; }
-                } else if (c.prev_me_stage_based_exit_th && s.lsad[0][l][r][reg] < ((uint32_t)c.prev_me_stage_based_exit_th >> 5)) {
-                    if (lane == 0) { s.lx[1][l][r][reg] = s.lx[0][l][r][reg]; s.ly[1][l][r][reg] = s.ly[0][l][r][reg]; s.lsad[1][l][r][reg] = s.lsad[0][l][r][reg]; }
-                } else {
-                    SvtB200SadSearchItem it;
-                    int16_t              o_x, o_y;
-                    hme_make_item(cur, rp, 1, c.hme_l1_w, c.hme_l1_h, c.hme_sub_sad, reg & 1, reg >> 1, bx, by, s.lx[0][l][r][reg], s.ly[0][l][r][reg], it, o_x, o_y);
-                    const SvtB200SadSearchResult q =
-                        sad_key_to_result(sad_search_warp((const uint8_t*)(uintptr_t)it.src_off, (const uint8_t*)(uintptr_t)it.ref_off, it, lane));
-                    int16_t  x, y;
-                    uint64_t sad;
-                    hme_finish_one(q, o_x, o_y, c.hme_sub_sad, 1, x, y, sad);
-                    if (lane == 0) { s.lx[1][l][r][reg] = x; s.ly[1][l][r][reg] = y; s.lsad[1][l][r][reg] = sad; }
+            __syncthreads();
+        }
+        if (stage == kPh1 && c.prehme_enable) {  // pre-HME reference pruning
+            if (threadIdx.x == 0) {
+                uint32_t best = kMaxU32;
+                for (int p = 0; p < n_pairs; p++) {
+                    const int l = pair_l(p), r = pair_r(p);
+                    if (!searched(c, l)) continue;
+                    best = min(best, (uint32_t)min(s.ph_sad[l][r][0], s.ph_sad[l][r][1]));
                 }
-                __syncwarp();
+                if (c.temporal_layer_index > 0 && best < (uint32_t)c.phme_sad_th)
+                    for (int p = 0; p < n_pairs; p++) {
+                        const int l = pair_l(p), r = pair_r(p);
+                        if (!s.do_ref[l][r] || r == 0) continue;
+                        const uint32_t ps = (uint32_t)min(s.ph_sad[l][r][0], s.ph_sad[l][r][1]);
+                        if ((uint32_t)((ps - best) * 100u) > (uint32_t)((uint32_t)c.phme_sad_pct * best)) s.do_ref[l][r] = 0;
+                    }
             }
-            // ---- level 2 (hme_level2_b64): no early exit, pruned references are searched as well
-            if (on && c.enable_l2 && searched(c, l)) {
-                if (c.prev_me_stage_based_exit_th && s.lsad[1][l][r][reg] < ((uint32_t)c.prev_me_stage_based_exit_th >> 2)) {
-                    if (lane == 0) { s.lx[2][l][r][reg] = s.lx[1][l][r][reg]; s.ly[2][l][r][reg] = s.ly[1][l][r][reg]; s.lsad[2][l][r][reg] = s.lsad[1][l][r][reg]; }
-                } else {
-                    SvtB200SadSearchItem it;
-                    int16_t              o_x, o_y;
-                    hme_make_item(cur, rp, 2, c.hme_l2_w, c.hme_l2_h, c.hme_sub_sad, reg & 1, reg >> 1, bx, by, s.lx[1][l][r][reg], s.ly[1][l][r][reg], it, o_x, o_y);
-                    const SvtB200SadSearchResult q =
-                        sad_key_to_result(sad_search_warp((const uint8_t*)(uintptr_t)it.src_off, (const uint8_t*)(uintptr_t)it.ref_off, it, lane));
-                    int16_t  x, y;
-                    uint64_t sad;
-                    hme_finish_one(q, o_x, o_y, c.hme_sub_sad, 2, x, y, sad);
-                    if (lane == 0) { s.lx[2][l][r][reg] = x; s.ly[2][l][r][reg] = y; s.lsad[2][l][r][reg] = sad; }
-                }
-                __syncwarp();
-            }
+            __syncthreads();
         }
     }
-    __syncthreads();
 
     // ---- set_final_seach_centre_sb + hme_prune_ref_and_adjust_sr (one thread: values carry over between references) ---------
     if (threadIdx.x == 0) {
@@ -534,78 +594,83 @@ me_b64_hme_kernel(const __grid_constant__ MeB64Table tab, int n_b64, int b64_w, 
     }
     __syncthreads();
 
-    // ---- integer_search_b64: the search window of every live reference; warp = reference ------------------------------------------
-    for (int p = warp; p < n_pairs; p += n_warps) {
-        const int l = pair_l(p), r = pair_r(p);
+    // ---- integer_search_b64: the search window of every live reference; warp = reference -------------------------------------------
+    static_assert(kHmeThreads / 32 >= 2 * kDepth, "one warp per reference");
+    if (warp < n_pairs) {
+        const int      p = warp, l = pair_l(p), r = pair_r(p);
+        const int16_t  org_x = s.org_x, org_y = s.org_y, blk_w = s.blk_w, blk_h = s.blk_h;
+        const uint8_t* src_full = block_src();
         const SvtB200MePicture& rp = tab.ref[l][r];
         const size_t item_idx = (size_t)p * n_b64 + b;
-        SvtB200FullpelItem it;
-        it.src_off = (uint64_t)(uintptr_t)src_full;
-        it.src_stride = (uint32_t)cur.stride[2];
-        it.ref_stride = (uint32_t)rp.stride[2];
-        it.sub_sad = (uint8_t)(c.me_sub_sad ? 1 : 0);
-        it.seeded = 0;
-        it.seed_x = it.seed_y = 0;
-        it.reserved[0] = it.reserved[1] = 0;
         const uint8_t* r0 = rp.plane[2] + (size_t)(rp.org_y[2] + org_y) * rp.stride[2] + rp.org_x[2] + org_x;  // zero-MV position
-        if (!s.do_ref[l][r]) {  // pruned: one position at the zero MV keeps the search kernel's item stream dense; the result is not used
-            it.ref_off = (uint64_t)(uintptr_t)r0;
-            it.sa_w = it.sa_h = 1;
-            it.org_x = it.org_y = 0;
-            if (lane == 0) items[item_idx] = it;
-            continue;
-        }
-        int16_t sx = s.sc_x[l][r], sy = s.sc_y[l][r];
-        const int dist = scaled_distance((int)(uint16_t)(int16_t)c.dist[l][r]);
-        int16_t sa_w = (int16_t)min(c.me_min_w * dist, c.me_max_w), sa_h = (int16_t)min(c.me_min_h * dist, c.me_max_h);
-        if (c.mvsa_enable && (!c.mvsa_nearest_ref_only || r == 0)) {
-            if (abs((int)sx) > c.mvsa_mv_size_th) sa_w = (int16_t)(sa_w * c.mvsa_multiplier);
-            if (abs((int)sy) > c.mvsa_mv_size_th) sa_h = (int16_t)(sa_h * c.mvsa_multiplier);
-        }
-        const int dv = (int)s.divisor[l][r];
-        sa_w = (int16_t)((max(1, sa_w / dv) + 7) & ~0x07);
-        sa_h = (int16_t)max(3, sa_h / dv);
-        if (c.me_early_exit_th) {
-            if (s.zz[l][r] < (uint32_t)c.me_early_exit_th / 6u) sa_w = sa_h = 1;
-        } else if ((sx != 0 || sy != 0) && c.is_ref) {
-            // check_00_center: keep the HME centre only if it beats the zero MV (SADs on every other row)
-            const int16_t RW = (int16_t)rp.width[2], RH = (int16_t)rp.height[2];
-            if ((int16_t)(org_x + sx) < -63) sx = (int16_t)(-63 - org_x);
-            if ((int16_t)(org_x + sx) > (int16_t)(RW - 1)) sx = (int16_t)(sx - ((org_x + sx) - (RW - 1)));
-            if ((int16_t)(org_y + sy) < -63) sy = (int16_t)(-63 - org_y);
-            if ((int16_t)(org_y + sy) > (int16_t)(RH - 1)) sy = (int16_t)(sy - ((org_y + sy) - (RH - 1)));
-            const uint32_t z = warp_sad_every_other_row(src_full, cur.stride[2], r0, rp.stride[2], blk_w, blk_h, lane) << 1;
-            const uint32_t h = warp_sad_every_other_row(src_full, cur.stride[2], r0 + (ptrdiff_t)sy * rp.stride[2] + sx, rp.stride[2], blk_w, blk_h, lane) << 1;
-            if (z <= h) sx = sy = 0;
-        }
-        // 8x8-SAD-variance probe at the search centre
-        if (c.var_enable && (int)sa_w * (int)sa_h > 24) {
-            const uint32_t var = warp_probe_sads(src_full, cur.stride[2], r0 + (ptrdiff_t)sy * rp.stride[2] + sx, rp.stride[2], c.me_sub_sad != 0,
-                                                 lane, seed_sad + item_idx * 85);
-            if (var > (uint32_t)c.var_mult2_th) {
-                sa_w = (int16_t)((max(1, sa_w * 3 / 2) + 7) & ~0x7);
-                sa_h = (int16_t)max(1, sa_h * 3 / 2);
+        // pruned: one position at the zero MV keeps the search kernel's item stream dense; the result is not used
+        int16_t sa_w = 1, sa_h = 1, ox = 0, oy = 0, sx = 0, sy = 0;
+        bool    seeded = false;
+        if (s.do_ref[l][r]) {
+            sx = s.sc_x[l][r];
+            sy = s.sc_y[l][r];
+            const int dist = scaled_distance((int)(uint16_t)(int16_t)c.dist[l][r]);
+            sa_w = (int16_t)min(c.me_min_w * dist, c.me_max_w);
+            sa_h = (int16_t)min(c.me_min_h * dist, c.me_max_h);
+            if (c.mvsa_enable && (!c.mvsa_nearest_ref_only || r == 0)) {
+                if (abs((int)sx) > c.mvsa_mv_size_th) sa_w = (int16_t)(sa_w * c.mvsa_multiplier);
+                if (abs((int)sy) > c.mvsa_mv_size_th) sa_h = (int16_t)(sa_h * c.mvsa_multiplier);
             }
-            if (var < (uint32_t)c.var_div4_th) {
-                sa_w = (int16_t)((max(1, sa_w >> 2) + 7) & ~0x7);
-                sa_h = (int16_t)max(3, max(1, sa_h >> 2));
-            } else if (var < (uint32_t)c.var_div2_th) {
-                sa_w = (int16_t)((min((int)sa_w, sa_w >> 1) + 7) & ~0x7);
-                sa_h = (int16_t)max(3, min((int)sa_h, sa_h >> 1));
+            const int dv = (int)s.divisor[l][r];
+            sa_w = (int16_t)((max(1, sa_w / dv) + 7) & ~0x07);
+            sa_h = (int16_t)max(3, sa_h / dv);
+            if (c.me_early_exit_th) {
+                if (s.zz[l][r] < (uint32_t)c.me_early_exit_th / 6u) sa_w = sa_h = 1;
+            } else if ((sx != 0 || sy != 0) && c.is_ref) {
+                // check_00_center: keep the HME centre only if it beats the zero MV (SADs on every other row)
+                const int16_t RW = (int16_t)rp.width[2], RH = (int16_t)rp.height[2];
+                if ((int16_t)(org_x + sx) < -63) sx = (int16_t)(-63 - org_x);
+                if ((int16_t)(org_x + sx) > (int16_t)(RW - 1)) sx = (int16_t)(sx - ((org_x + sx) - (RW - 1)));
+                if ((int16_t)(org_y + sy) < -63) sy = (int16_t)(-63 - org_y);
+                if ((int16_t)(org_y + sy) > (int16_t)(RH - 1)) sy = (int16_t)(sy - ((org_y + sy) - (RH - 1)));
+                const uint32_t z = warp_sad_every_other_row(src_full, cur.stride[2], r0, rp.stride[2], blk_w, blk_h, lane) << 1;
+                const uint32_t h = warp_sad_every_other_row(src_full, cur.stride[2], r0 + (ptrdiff_t)sy * rp.stride[2] + sx, rp.stride[2], blk_w, blk_h, lane) << 1;
+                if (z <= h) sx = sy = 0;
             }
-            it.seeded = 1;
-            it.seed_x = sx;
-            it.seed_y = sy;
+            // 8x8-SAD-variance probe at the search centre
+            if (c.var_enable && (int)sa_w * (int)sa_h > 24) {
+                const uint32_t var = warp_probe_sads(src_full, cur.stride[2], r0 + (ptrdiff_t)sy * rp.stride[2] + sx, rp.stride[2], c.me_sub_sad != 0,
+                                                     lane, seed_sad + item_idx * 85);
+                if (var > (uint32_t)c.var_mult2_th) {
+                    sa_w = (int16_t)((max(1, sa_w * 3 / 2) + 7) & ~0x7);
+                    sa_h = (int16_t)max(1, sa_h * 3 / 2);
+                }
+                if (var < (uint32_t)c.var_div4_th) {
+                    sa_w = (int16_t)((max(1, sa_w >> 2) + 7) & ~0x7);
+                    sa_h = (int16_t)max(3, max(1, sa_h >> 2));
+                } else if (var < (uint32_t)c.var_div2_th) {
+                    sa_w = (int16_t)((min((int)sa_w, sa_w >> 1) + 7) & ~0x7);
+                    sa_h = (int16_t)max(3, min((int)sa_h, sa_h >> 1));
+                }
+                seeded = true;
+            }
+            ox = (int16_t)(sx - (sa_w >> 1));
+            oy = (int16_t)(sy - (sa_h >> 1));
+            clip_search_area(org_x, ox, sa_w, 63, (int16_t)aw, true);  // against the 8-aligned picture size (:3093-3100)
+            clip_search_area(org_y, oy, sa_h, 63, (int16_t)ah, false);
         }
-        int16_t ox = (int16_t)(sx - (sa_w >> 1)), oy = (int16_t)(sy - (sa_h >> 1));
-        clip_search_area(org_x, ox, sa_w, 63, (int16_t)aw, true);  // against the 8-aligned picture size (:3093-3100)
-        clip_search_area(org_y, oy, sa_h, 63, (int16_t)ah, false);
-        it.ref_off = (uint64_t)(uintptr_t)(r0 + (ptrdiff_t)oy * rp.stride[2] + ox);
-        it.sa_w = sa_w;
-        it.sa_h = sa_h;
-        it.org_x = ox;
-        it.org_y = oy;
-        if (lane == 0) items[item_idx] = it;
+        if (lane == 0) {
+            SvtB200FullpelItem it;
+            it.src_off = (uint64_t)(uintptr_t)src_full;
+            it.ref_off = (uint64_t)(uintptr_t)(r0 + (ptrdiff_t)oy * rp.stride[2] + ox);
+            it.src_stride = (uint32_t)cur.stride[2];
+            it.ref_stride = (uint32_t)rp.stride[2];
+            it.sa_w = sa_w;
+            it.sa_h = sa_h;
+            it.org_x = ox;
+            it.org_y = oy;
+            it.sub_sad = (uint8_t)(c.me_sub_sad ? 1 : 0);
+            it.seeded = seeded ? 1 : 0;
+            it.seed_x = seeded ? sx : (int16_t)0;
+            it.seed_y = seeded ? sy : (int16_t)0;
+            it.reserved[0] = it.reserved[1] = 0;
+            items[item_idx] = it;
+        }
     }
     // state for the finishing kernel + diagnostics
     if (threadIdx.x < 2 * kDepth) {
@@ -876,12 +941,7 @@ extern "C" int svt_b200_me_b64_picture_dev(const SvtB200MePicture* cur, const Sv
     B200_CUDA_CHECK(cudaMemsetAsync(out->total_me_candidate_index, 0, (size_t)n_b64 * n_pu, st));
     B200_CUDA_CHECK(cudaMemsetAsync(out->me_candidate_array, 0, (size_t)n_b64 * n_pu * c.max_cand, st));
     B200_CUDA_CHECK(cudaMemsetAsync(out->me_mv_array, 0, (size_t)n_b64 * n_pu * c.max_refs * 4, st));
-    // two references of a block in flight per CTA pays off with many references and costs with few (chosen on the previous target
-    // GPU; not re-measured on H100)
-    if (n_refs >= 6)
-        me_b64_hme_kernel<2><<<n_b64, 256, 0, st>>>(tab, n_b64, b64_w, w->items, w->seed, w->do_ref, out->hme_centre, out->zz_sad);
-    else
-        me_b64_hme_kernel<1><<<n_b64, 128, 0, st>>>(tab, n_b64, b64_w, w->items, w->seed, w->do_ref, out->hme_centre, out->zz_sad);
+    me_b64_hme_kernel<<<n_b64, kHmeThreads, 0, st>>>(tab, n_b64, b64_w, w->items, w->seed, w->do_ref, out->hme_centre, out->zz_sad);
     B200_LAUNCH_CHECK();
     if (!launch_fullpel_tma(cur, refs, n_refs, n_b64, w->items, pairs, out->best_sad, out->best_mv, st, w->seed)) {
         fprintf(stderr, "[svt_b200] svt_b200_me_b64_picture_dev: the luma planes do not meet the layout rule (16-byte aligned base and pitch)\n");

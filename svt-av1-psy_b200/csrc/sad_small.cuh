@@ -20,6 +20,7 @@ constexpr int kSmallSearchMaxPos = 256;  // searches with at most this many posi
 struct ByteRun {
     const uint32_t* w;
     int shift, last;
+    ByteRun() = default;
     __device__ __forceinline__ ByteRun(const uint8_t* p, int n) {
         const uintptr_t a = reinterpret_cast<uintptr_t>(p);
         w     = reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3));
@@ -67,6 +68,8 @@ __device__ __forceinline__ void sad_load_run(const uint8_t* p, int nbytes, uint3
     for (int j = 0; j < 6; j++) out[j] = __funnelshift_r(w[j], w[j + 1], shift);
 }
 
+// ONE_ROW: the block has at most 32 units, so a lane owns a single block row and keeps its source words for the whole search
+template <bool ONE_ROW>
 __device__ __forceinline__ unsigned long long sad_search_warp_w16(const uint8_t* __restrict__ src0, const uint8_t* __restrict__ ref0,
                                                                   const SvtB200SadSearchItem& item, int lane) {
     const int bw = item.block_w, bh = item.block_h, sa_w = item.sa_w, sa_h = item.sa_h;
@@ -83,6 +86,8 @@ __device__ __forceinline__ unsigned long long sad_search_warp_w16(const uint8_t*
     const uint8_t* src_u = src0 + (size_t)r_first * item.src_stride + 16 * c;  // this lane's first unit
     const uint8_t* ref_u = ref0 + (size_t)r_first * item.ref_stride + 16 * c;
     const size_t   src_adv = (size_t)r_step * item.src_stride, ref_adv = (size_t)r_step * item.ref_stride;
+    uint32_t sw1[6];
+    if (ONE_ROW && r_first < bh) sad_load_run<16>(src_u, 16, sw1);
     unsigned long long best = ~0ull;
     int y = 0, xt = grp;  // this group's tile, advanced by `groups` tiles per round
     while (xt >= xtiles) { xt -= xtiles; y++; }
@@ -98,9 +103,14 @@ __device__ __forceinline__ unsigned long long sad_search_warp_w16(const uint8_t*
         if (line_on) {
             const uint8_t* ps = src_u;
             const uint8_t* pr = ref_u + (size_t)yy * item.ref_step + x0;
-            for (int r = r_first; r < bh; r += r_step, ps += src_adv, pr += ref_adv) {
+            for (int r = r_first; r < (ONE_ROW ? min(bh, r_first + 1) : bh); r += r_step, ps += src_adv, pr += ref_adv) {
                 uint32_t sw[6], rw[6];
-                sad_load_run<16>(ps, 16, sw);
+                if (ONE_ROW) {
+#pragma unroll
+                    for (int k = 0; k < 4; k++) sw[k] = sw1[k];
+                } else {
+                    sad_load_run<16>(ps, 16, sw);
+                }
                 sad_load_run<16>(pr, 16 + npos - 1, rw);
 #pragma unroll
                 for (int i = 0; i < 8; i++) {
@@ -162,18 +172,23 @@ __device__ __forceinline__ unsigned long long sad_search_warp_w16(const uint8_t*
     return best;
 }
 
-// all 32 lanes call; every lane returns the winning key (~0ull when no position qualifies)
+// all 32 lanes call; every lane returns the winning key (~0ull when no position qualifies).  YG: search rows the narrow-block
+// path evaluates per pass over the source block; fewer rows reload the source words more often but hold fewer registers
+// (2 keeps a caller bounded to 64 registers free of spills).
+template <int YG = 4>
 __device__ __forceinline__ unsigned long long sad_search_warp(const uint8_t* __restrict__ src0, const uint8_t* __restrict__ ref0,
                                                               const SvtB200SadSearchItem& item, int lane) {
     const int bw = item.block_w, bh = item.block_h, sa_w = item.sa_w, sa_h = item.sa_h;
     unsigned long long best = ~0ull;
     if (sa_w <= 0 || sa_h <= 0 || bw <= 0 || bh <= 0) return best;
-    if (bw == 16 || bw == 32 || bw == 64) return sad_search_warp_w16(src0, ref0, item, lane);
+    if (bw == 16 || bw == 32 || bw == 64) {
+        const int units = bh << (bw == 64 ? 2 : (bw == 32 ? 1 : 0));
+        return units <= 32 ? sad_search_warp_w16<true>(src0, ref0, item, lane) : sad_search_warp_w16<false>(src0, ref0, item, lane);
+    }
     const bool     skip = (bw == 16 && bh <= 16 && item.skip_search_line);
     const int      xs = lane & 7, slice = lane >> 3;
     const int      nw = (bw + 3) >> 2, tail = bw & 3;
     const uint32_t tailmask = tail ? ((1u << (tail * 8)) - 1u) : 0xffffffffu;
-    constexpr int  YG = 4;  // search rows evaluated per pass over the source block (the loop body below is written for 4)
     for (int y0 = 0; y0 < sa_h; y0 += YG) {
         for (int x0 = 0; x0 < sa_w; x0 += 8) {
             const bool valid = x0 + xs < sa_w;
@@ -185,32 +200,33 @@ __device__ __forceinline__ unsigned long long sad_search_warp(const uint8_t* __r
                 const ByteRun  S(src0 + (size_t)r * item.src_stride, bw);
                 const uint8_t* rrow = ref0 + (size_t)r * item.ref_stride + x;
                 // rows past the area repeat the last one; their sums are dropped below
-                const ByteRun R0(rrow + (size_t)min(y0 + 0, sa_h - 1) * item.ref_step, bw), R1(rrow + (size_t)min(y0 + 1, sa_h - 1) * item.ref_step, bw),
-                    R2(rrow + (size_t)min(y0 + 2, sa_h - 1) * item.ref_step, bw), R3(rrow + (size_t)min(y0 + 3, sa_h - 1) * item.ref_step, bw);
-                uint32_t slo = S.raw(0), r0 = R0.raw(0), r1 = R1.raw(0), r2 = R2.raw(0), r3 = R3.raw(0);
+                ByteRun  R[YG];
+                uint32_t rlo[YG];
+#pragma unroll
+                for (int k = 0; k < YG; k++) {
+                    R[k]   = ByteRun(rrow + (size_t)min(y0 + k, sa_h - 1) * item.ref_step, bw);
+                    rlo[k] = R[k].raw(0);
+                }
+                uint32_t slo = S.raw(0);
                 // all words but the last: the next aligned word always holds valid bytes, nothing to mask
 #pragma unroll 4
                 for (int j = 0; j < nw - 1; j++) {
-                    const uint32_t shi = __ldg(S.w + j + 1), h0 = __ldg(R0.w + j + 1), h1 = __ldg(R1.w + j + 1), h2 = __ldg(R2.w + j + 1),
-                                   h3 = __ldg(R3.w + j + 1);
-                    const uint32_t sv = __funnelshift_r(slo, shi, S.shift);  // one source word against four search rows
-                    acc[0] = __vsadu4(sv, __funnelshift_r(r0, h0, R0.shift)) + acc[0];
-                    acc[1] = __vsadu4(sv, __funnelshift_r(r1, h1, R1.shift)) + acc[1];
-                    acc[2] = __vsadu4(sv, __funnelshift_r(r2, h2, R2.shift)) + acc[2];
-                    acc[3] = __vsadu4(sv, __funnelshift_r(r3, h3, R3.shift)) + acc[3];
+                    const uint32_t shi = __ldg(S.w + j + 1);
+                    const uint32_t sv = __funnelshift_r(slo, shi, S.shift);  // one source word against YG search rows
+#pragma unroll
+                    for (int k = 0; k < YG; k++) {
+                        const uint32_t h = __ldg(R[k].w + j + 1);
+                        acc[k] = __vsadu4(sv, __funnelshift_r(rlo[k], h, R[k].shift)) + acc[k];
+                        rlo[k] = h;
+                    }
                     slo = shi;
-                    r0  = h0;
-                    r1  = h1;
-                    r2  = h2;
-                    r3  = h3;
                 }
                 {  // last word: the following aligned word may lie past the row (clamped index), bytes past bw are masked
-                    const uint32_t shi = S.raw(nw), h0 = R0.raw(nw), h1 = R1.raw(nw), h2 = R2.raw(nw), h3 = R3.raw(nw);
-                    const uint32_t sv = __funnelshift_r(slo, shi, S.shift) & tailmask;
-                    acc[0] = __vsadu4(sv, __funnelshift_r(r0, h0, R0.shift) & tailmask) + acc[0];
-                    acc[1] = __vsadu4(sv, __funnelshift_r(r1, h1, R1.shift) & tailmask) + acc[1];
-                    acc[2] = __vsadu4(sv, __funnelshift_r(r2, h2, R2.shift) & tailmask) + acc[2];
-                    acc[3] = __vsadu4(sv, __funnelshift_r(r3, h3, R3.shift) & tailmask) + acc[3];
+                    const uint32_t sv = __funnelshift_r(slo, S.raw(nw), S.shift) & tailmask;
+#pragma unroll
+                    for (int k = 0; k < YG; k++) {
+                        acc[k] = __vsadu4(sv, __funnelshift_r(rlo[k], R[k].raw(nw), R[k].shift) & tailmask) + acc[k];
+                    }
                 }
             }
 #pragma unroll

@@ -1,14 +1,15 @@
 #!/usr/bin/env python3
 """Per-class timing of the transform kernel (txfm_kernel<Chain / Forward / Inverse, 4..64>) and the bench figures next to it.
 
-    python tools/profile_trio.py [--configs 1 2] [--steps 20] [--out DIR]
+    python tools/profile_trio.py [--configs 1 2] [--steps 20] [--out DIR] [--kernels me_b64 fullpel_search]
     python tools/profile_trio.py --bench-runs 3 --bench-trees . ../other_checkout [--bench-config 1]
 
 Profile mode: frames of each configuration through the hot path with every call in order on one stream, under
 torch.profiler (CUDA activities); one line per trio kernel -- name, grid, launches, mean us -- and the other calls'
 kernels summed per call, with the card's name and power limit; then the separate calls (residual, forward, quantise,
-inverse) on the same frame, one line per forward and inverse kernel.  The traces go to DIR (default: a temporary
-directory).  Bench mode: `bench.py --gpus 1 --steps 3000 --warmup 50 --no-cpu-baseline` run alternately from each
+inverse) on the same frame, one line per forward and inverse kernel.  With --kernels, one line per kernel whose name
+contains one of the given strings, in place of the trio lines (e.g. `--kernels me_b64 fullpel_search` splits the
+me_search call).  The traces go to DIR (default: a temporary directory).  Bench mode: `bench.py --gpus 1 --steps 3000 --warmup 50 --no-cpu-baseline` run alternately from each
 tree, `value` and `calls_ms` printed per run.  The two modes are separate processes: the profiler slows the host."""
 import argparse
 import json
@@ -29,7 +30,7 @@ def card():
         return "unknown card (%s)" % e
 
 
-def profile(configs, steps, out_dir):
+def profile(configs, steps, out_dir, kernels=None):
     sys.path.insert(0, ROOT)
     import torch
     from torch.profiler import ProfilerActivity, profile as tprofile
@@ -55,6 +56,11 @@ def profile(configs, steps, out_dir):
         prof.export_chrome_trace(trace)
         kern = kernel_times(trace)
         print("config %d: %d profiled steps" % (cfg, steps))
+        if kernels:
+            for k in kernels:
+                print_classes(kern, k)
+            sys.stdout.flush()
+            continue
         print_classes(kern, "txfm_kernel<Chain")
         per = {}
         for (s, g), (n, t) in kern.items():
@@ -100,8 +106,8 @@ def kernel_times(trace):
     return kern
 
 
-def print_classes(kern, prefix):
-    rows = sorted(((s, g, n, t) for (s, g), (n, t) in kern.items() if s.startswith(prefix)), key=lambda x: -x[3] / x[2])
+def print_classes(kern, pattern):
+    rows = sorted(((s, g, n, t) for (s, g), (n, t) in kern.items() if pattern in s), key=lambda x: -x[3] / x[2])
     for s, g, n, t in rows:
         print("  %-60s grid=%-14s launches=%-5d mean=%8.2f us" % (s, "x".join(map(str, g)), n, t / n))
 
@@ -133,6 +139,8 @@ def main():
     ap.add_argument("--configs", type=int, nargs="+", default=[1, 2])
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--out", default=None, help="directory for the profiler traces (default: a temporary directory)")
+    ap.add_argument("--kernels", nargs="+", default=None,
+                    help="profile mode: print only the kernels whose names contain one of these strings (default: the trio)")
     ap.add_argument("--bench-runs", type=int, default=0)
     ap.add_argument("--bench-trees", nargs="+", default=[ROOT])
     ap.add_argument("--bench-config", type=int, default=1)
@@ -144,10 +152,10 @@ def main():
         return
     if a.out:
         os.makedirs(a.out, exist_ok=True)
-        profile(a.configs, a.steps, a.out)
+        profile(a.configs, a.steps, a.out, a.kernels)
     else:
         with tempfile.TemporaryDirectory() as d:
-            profile(a.configs, a.steps, d)
+            profile(a.configs, a.steps, d, a.kernels)
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """The open-loop ME call alone (pyramid + complete driver) for `compute-sanitizer --tool memcheck|racecheck python
-tools/sanitize_me.py`: preset 8 (4 references: one reference of a block at a time in me_b64_hme_kernel) and preset 4
-(7 references: two at a time).  Drives only the product library."""
+tools/sanitize_me.py`: preset 8 (4 references) and preset 4 (7 references: every pre-HME and HME stage of
+me_b64_hme_kernel has more warp jobs than the CTA has warps).  Drives only the product library."""
 import os
 import sys
 
