@@ -12,11 +12,12 @@
 // per row in the row pass, each running the generated straight-line network on its vector in registers
 // (txfm_tables.cuh).  In the 32- and 64-point classes a block has a CTA of 2 * max(W,H) threads to itself, and its
 // 32- and 64-point vectors run split across two lanes.  The block sits in shared memory in element-major order with
-// an odd pitch, so the passes and the transposing hand-over are bank-conflict free; residual loads / coefficient
-// stores are coalesced rows.
+// an odd pitch, so the passes and the transposing hand-over are bank-conflict free; pixel, residual and coefficient
+// rows move between global memory and the planes in 4- to 16-byte words where the item's origin and stride allow it.
 #include <map>
 #include <mutex>
 #include <type_traits>
+#include <utility>
 #include "txfm_tables.cuh"
 #include "quant_one.cuh"
 #include "../../include/svt_b200.h"
@@ -49,12 +50,6 @@ __host__ __device__ constexpr int team_stride(int team) {
     return team == 4 ? 68 : (team == 8 ? 152 : (team == 16 ? 560 : 2 * team * (team + 1)));
 }
 
-__host__ __device__ inline int rect_log_ratio(int w, int h) {  // get_rect_tx_log_ratio
-    if (w == h) return 0;
-    if (w > h) return w == 2 * h ? 1 : (w == 4 * h ? 2 : 3);
-    return h == 2 * w ? -1 : (h == 4 * w ? -2 : -3);
-}
-
 // ------------------------------------------------------------------------------------------------
 // One block body for the three batch calls, as the modes of txfm_kernel:
 //   Forward (svt_b200_fwd_txfm_batch_dev): residual -> coefficients;
@@ -63,6 +58,8 @@ __host__ __device__ inline int rect_log_ratio(int w, int h) {  // get_rect_tx_lo
 //           -> quantise -> inverse transform + reconstruction without leaving shared memory: the coefficients and the
 //           dequantised levels never travel through HBM between the steps.
 // The fused calls are bit-identical to the separate ones because each step is the same code in every mode.
+// The body is a template on the transform size (txfm_block<..., SZ>): every element loop has a constant trip count and
+// constant index arithmetic.  A class launch holds the bodies of its sizes and picks one per item (dispatch_size).
 // ------------------------------------------------------------------------------------------------
 struct Forward { using Item = SvtB200FwdTxfmItem; };
 struct Inverse { using Item = SvtB200InvTxfmItem; };
@@ -77,217 +74,398 @@ __device__ __forceinline__ const SvtB200InvTxfmItem& inv_part(const SvtB200TrioI
 template <class I> __device__ __forceinline__ const auto& shape_part(const I& i) { return fwd_part(i); }
 
 // the forward's last steps on one coefficient: final shift, then the scaling of 2:1 rectangles
-__device__ __forceinline__ int32_t fwd_out(int32_t v, const TxCfg& cfg, int rect) {
+template <int RECT>
+__device__ __forceinline__ int32_t fwd_out(int32_t v, const TxCfg& cfg) {
     v = round_shift_arr(v, -cfg.f_s2);
-    if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewSqrt2, 12);
+    if constexpr (RECT == 1 || RECT == -1) v = round_shift64((long long)v * kNewSqrt2, 12);
     return v;
 }
 // the inverse's first steps on one dequantised coefficient: the scaling of 2:1 rectangles, then the row clamp
-__device__ __forceinline__ int32_t inv_in(int32_t v, int rect, int row_clamp) {
-    if (rect == 1 || rect == -1) v = round_shift64((long long)v * kNewInvSqrt2, 12);
+template <int RECT>
+__device__ __forceinline__ int32_t inv_in(int32_t v, int row_clamp) {
+    if constexpr (RECT == 1 || RECT == -1) v = round_shift64((long long)v * kNewInvSqrt2, 12);
     return clamp_bits(v, row_clamp);
 }
 
 // A 1-D pass.  In the 32- and 64-point classes (one block per CTA of 2 * TEAM threads) 32- and 64-point vectors run split
 // across two lanes, shorter ones one per thread.  FULL64: 64-point vectors run whole on one thread, so that all 64 outputs
 // exist (the forward batch's unpacked items); otherwise the 64-point networks are the packed ones.
-template <int TEAM, int THREADS, bool INV, bool FULL64>
-__device__ __forceinline__ void txfm_pass(int type, int32_t* x, int N, int V, int P, int cos_bit, int clampb, int tid) {
-    if constexpr (TEAM >= 32) {
+template <int TEAM, int THREADS, bool INV, bool FULL64, int N, int V, int P>
+__device__ __forceinline__ void txfm_pass(int type, int32_t* x, int cos_bit, int clampb, int tid) {
+    if constexpr (TEAM >= 32 && N == 32) {
         static_assert(THREADS == 2 * TEAM, "a lane pair per vector");
-        if (N == 32) return txfm_pass_split<32, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
-        if constexpr (TEAM >= 64 && !FULL64) {
-            if (N == 64) return txfm_pass_split<64, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
-        }
+        return txfm_pass_split<32, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
+    } else if constexpr (TEAM >= 64 && N == 64 && !FULL64) {
+        return txfm_pass_split<64, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
+    } else {
+        txfm_pass_1d<TEAM, INV, !FULL64>(type, x, N, V, P, cos_bit, clampb, tid);
     }
-    txfm_pass_1d<TEAM, INV, !FULL64>(type, x, N, V, P, cos_bit, clampb, tid);
 }
 
-template <class M, int TEAM, int THREADS, typename PIX>
-__global__ void __launch_bounds__(THREADS)
-txfm_kernel(const int16_t* __restrict__ src_base, const PIX* __restrict__ srcpix_base /*Chain, non-null: residual = source - prediction, formed here*/,
-            const PIX* __restrict__ pred_base, PIX* __restrict__ recon_base,
-            int32_t* __restrict__ coef_base /*Forward: the coefficients; Chain: the quantised levels*/,
-            int32_t* __restrict__ dq_base /*Chain: the dequantised levels, may be null*/, const int16_t* __restrict__ iscan_base,
-            const uint8_t* __restrict__ qm_base, const typename M::Item* __restrict__ items, int n_items, uint16_t* __restrict__ eobs,
-            const int32_t* __restrict__ dq_in /*Inverse: the dequantised coefficients*/) {
+// ---- element loops -------------------------------------------------------------------------------------------------
+// The words of V elements of a region of R rows of W elements, spread over the MOVERS threads of a team: f(r, c) for
+// every word this thread moves (c: the word's first column).  Trip count and index split are constants.
+template <int W, int R, int V, int MOVERS, class F>
+__device__ __forceinline__ void for_words(int tid, F&& f) {
+    static_assert(W % V == 0, "whole words per row");
+    constexpr int PER_ROW = W / V, N = PER_ROW * R;
+#pragma unroll 2
+    for (int k = 0; k < (N + MOVERS - 1) / MOVERS; k++) {
+        const int w = tid + k * MOVERS;
+        if (N % MOVERS == 0 || w < N) f(w / PER_ROW, (w % PER_ROW) * V);
+    }
+}
+
+// V consecutive elements of global memory: one 4-, 8- or 16-byte word when VEC (the caller has checked the alignment:
+// row_words), V element moves otherwise
+template <int V, typename T> union Word {
+    using U = std::conditional_t<V * sizeof(T) == 4, uint32_t, std::conditional_t<V * sizeof(T) == 8, uint2, uint4>>;
+    static_assert(V * sizeof(T) == 4 || V * sizeof(T) == 8 || V * sizeof(T) == 16, "a word is 4, 8 or 16 bytes");
+    U u;
+    T e[V];
+};
+template <bool VEC, int V, typename T>
+__device__ __forceinline__ void ld_word(const T* p, T (&v)[V]) {
+    if constexpr (VEC) {
+        Word<V, T> w;
+        w.u = *reinterpret_cast<const typename Word<V, T>::U*>(p);
+#pragma unroll
+        for (int j = 0; j < V; j++) v[j] = w.e[j];
+    } else {
+#pragma unroll
+        for (int j = 0; j < V; j++) v[j] = p[j];
+    }
+}
+template <bool VEC, int V, typename T>
+__device__ __forceinline__ void st_word(T* p, const T (&v)[V]) {
+    if constexpr (VEC) {
+        Word<V, T> w;
+#pragma unroll
+        for (int j = 0; j < V; j++) w.e[j] = v[j];
+        *reinterpret_cast<typename Word<V, T>::U*>(p) = w.u;
+    } else {
+#pragma unroll
+        for (int j = 0; j < V; j++) p[j] = v[j];
+    }
+}
+// the rows of a block starting at p with the given stride (in elements) can move in words of V elements.  A per-item,
+// hence team-uniform, predicate: the block's origin and its stride are whole words.
+template <int V, typename T>
+__device__ __forceinline__ bool row_words(const T* p, size_t stride) {
+    constexpr int BYTES = V * (int)sizeof(T);
+    return ((uintptr_t)p % BYTES) == 0 && (stride * sizeof(T)) % BYTES == 0;
+}
+// runs f(std::true_type) or f(std::false_type): the word or the element form of a loop
+template <class F> __device__ __forceinline__ void with_words(bool vec, F&& f) {
+    if (vec) f(std::true_type{});
+    else f(std::false_type{});
+}
+// the word widths: pixels and residual samples up to 16 bytes and at most a row; coefficients, levels, scan positions
+// and matrix weights 4 at a time (int4, 4 x int16, u32)
+template <int W, typename T> constexpr int kRowWord = W < 16 / (int)sizeof(T) ? W : 16 / (int)sizeof(T);
+constexpr int kCoefWord = 4;
+
+// the device buffers of a batch call, in txfm_kernel's order; each mode uses its own
+template <typename PIX>
+struct TxfmPtrs {
+    const int16_t* src_base;    // residual (Forward; Chain without source)
+    const PIX*     srcpix_base; // Chain, non-null: residual = source - prediction, formed here
+    const PIX*     pred_base;
+    PIX*           recon_base;
+    int32_t*       coef_base;   // Forward: the coefficients; Chain: the quantised levels
+    int32_t*       dq_base;     // Chain: the dequantised levels, may be null
+    const int16_t* iscan_base;
+    const uint8_t* qm_base;
+    uint16_t*      eobs;
+    const int32_t* dq_in;       // Inverse: the dequantised coefficients
+};
+
+// One block of size SZ.  A and B: the team's two shared-memory planes.
+template <class M, int TEAM, int THREADS, typename PIX, int SZ>
+__device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typename M::Item& item, int it, int32_t* A, int32_t* B,
+                                           int tid, int& s_eob) {
     constexpr bool FWD = !std::is_same_v<M, Inverse>, INV = !std::is_same_v<M, Forward>, CHAIN = FWD && INV;
+    constexpr bool SOLO = TEAM >= 32;
+    constexpr int  MOVERS = SOLO ? THREADS : TEAM;
+    constexpr int  W = tx_w(SZ), H = tx_h(SZ);
+    static_assert((W > H ? W : H) == TEAM, "a size runs in the team class of its longer side");
+    constexpr int  RECT = W == H ? 0 : (W > H ? (W == 2 * H ? 1 : (W == 4 * H ? 2 : 3)) : (H == 2 * W ? -1 : (H == 4 * W ? -2 : -3)));  // get_rect_tx_log_ratio
+    constexpr int  Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;  // 64-point dimensions are packed (inv_transforms.c:2567-2686)
+    constexpr int  PW = W + 1, PH = H + 1;  // odd pitches: a plane holds the block as [r * PW + c] or as [c * PH + r]
+    constexpr int  VP = kRowWord<W, PIX>, VR = kRowWord<W, int16_t>, VC = kCoefWord;
+    const auto&    fi  = fwd_part(item);
+    const TxCfg    cfg = c_txcfg[SZ][shape_part(item).tx_type];
+    int            bd  = 0;
+    if constexpr (INV) bd = inv_part(item).bd;
+    if constexpr (FWD) {  // ---- forward transform (transforms.c:2286-2318) ----
+        const size_t sstride = fi.src_stride;
+        // load, optional up/down flip, pre-shift
+        bool from_source = false;
+        if constexpr (CHAIN) from_source = g.srcpix_base != nullptr;
+        if constexpr (CHAIN) if (from_source) {  // svt_aom_residual_kernel fused in: the source picture shares the residual plane's geometry
+            const PIX*   sp = g.srcpix_base + fi.src_off;
+            const PIX*   pp = g.pred_base + item.inv.pred_off;
+            const size_t pstride = item.inv.pred_stride;
+            with_words(row_words<VP>(sp, sstride) && row_words<VP>(pp, pstride), [&](auto vec) {
+                for_words<W, H, VP, MOVERS>(tid, [&](int r, int c) {
+                    const int rr = cfg.f_ud ? (H - 1 - r) : r;
+                    PIX s[VP], p[VP];
+                    ld_word<decltype(vec)::value>(sp + rr * sstride + c, s);
+                    ld_word<decltype(vec)::value>(pp + rr * pstride + c, p);
+#pragma unroll
+                    for (int j = 0; j < VP; j++) A[r * PW + c + j] = round_shift_arr((int32_t)s[j] - (int32_t)p[j], -cfg.f_s0);
+                });
+            });
+        }
+        if (!from_source) {
+            const int16_t* src = g.src_base + fi.src_off;
+            with_words(row_words<VR>(src, sstride), [&](auto vec) {
+                for_words<W, H, VR, MOVERS>(tid, [&](int r, int c) {
+                    const int rr = cfg.f_ud ? (H - 1 - r) : r;
+                    int16_t   s[VR];
+                    ld_word<decltype(vec)::value>(src + rr * sstride + c, s);
+#pragma unroll
+                    for (int j = 0; j < VR; j++) A[r * PW + c + j] = round_shift_arr((int32_t)s[j], -cfg.f_s0);
+                });
+            });
+        }
+        team_sync<TEAM, SOLO>();
+        // columns: vector v = column v (Chain: rows >= Hp of the result are not needed)
+        txfm_pass<TEAM, THREADS, false, !INV, H, W, PW>(cfg.f_tc, A, cfg.f_cbc, 0, tid);
+        team_sync<TEAM, SOLO>();
+        // round-shift, optional left/right flip, hand over transposed (element = column); Chain: only the Hp rows that
+        // survive the packing
+        constexpr int Hk = INV ? Hp : H;
+        for_words<W, Hk, 1, MOVERS>(tid, [&](int r, int c) {
+            const int cc = cfg.f_lr ? (W - 1 - c) : c;
+            B[cc * PH + r] = round_shift_arr(A[r * PW + c], -cfg.f_s1);
+        });
+        team_sync<TEAM, SOLO>();
+        txfm_pass<TEAM, THREADS, false, !INV, W, Hk, PH>(cfg.f_tr, B, cfg.f_cbr, 0, tid);  // rows: vector v = row v
+        team_sync<TEAM, SOLO>();
+    }
+    if constexpr (!INV) {  // ---- Forward: the coefficients out ----
+        int32_t*  dst = g.coef_base + fi.dst_off;
+        const int part_shift = (fi.reserved >> 1) & 3;  // 0 full, 1 = N2, 2 = N4
+        const int keep_h = max(H >> part_shift, 1), keep_w = max(W >> part_shift, 1);
+        // WO x HO coefficients in rows of WO: packed output keeps the top-left min(W,32) x min(H,32) (svt_handle_transform64x64
+        // repack, transforms.c:2374), otherwise all of them
+        auto out = [&](auto vec, auto wo, auto ho) {
+            constexpr int WO = decltype(wo)::value, HO = decltype(ho)::value;
+            for_words<WO, HO, VC, MOVERS>(tid, [&](int r, int c) {
+                int32_t v[VC];
+#pragma unroll
+                for (int j = 0; j < VC; j++) {
+                    v[j] = fwd_out<RECT>(B[(c + j) * PH + r], cfg);
+                    // N2 / N4 (av1_tranform_two_d_core_N2_c / _N4_c, transforms.c:5202, 6769): the top-left half / quarter
+                    // of every dimension, identical to the full transform's values there, zero everywhere else
+                    if (part_shift && (r >= keep_h || c + j >= keep_w)) v[j] = 0;
+                }
+                st_word<decltype(vec)::value>(dst + r * WO + c, v);
+            });
+        };
+        with_words(row_words<VC>(dst, 0), [&](auto vec) {
+            if ((fi.reserved & 1) && (W != Wp || H != Hp)) out(vec, std::integral_constant<int, Wp>{}, std::integral_constant<int, Hp>{});
+            else out(vec, std::integral_constant<int, W>{}, std::integral_constant<int, H>{});
+        });
+        team_sync<TEAM, SOLO>();
+    } else {
+        // the inverse's input plane, rows first: A[c * PH + r], element = column, vector = row; zero outside the packed
+        // Wp x Hp, which the passes keep zero
+        const auto& ii = inv_part(item);
+        const int   row_clamp = bd + 8;
+        int eob = 0;
+        if constexpr (CHAIN) {  // ---- quantise the (packed) coefficients; the dequantised levels are the input ----
+            const SvtB200QuantItem& qi = item.quant;
+            const QuantK   k   = quant_consts(qi);
+            const uint8_t* qm  = qi.qm_off == SVT_B200_NO_QM ? nullptr : g.qm_base + qi.qm_off;
+            const uint8_t* iqm = qi.iqm_off == SVT_B200_NO_QM ? nullptr : g.qm_base + qi.iqm_off;
+            const int16_t* iscan = g.iscan_base + qi.scan_off;
+            int32_t*       qc = g.coef_base + qi.q_off;
+            int32_t*       dqc = g.dq_base ? g.dq_base + qi.dq_off : nullptr;
+            if (SOLO && threadIdx.x == 0) s_eob = 0;
+            const bool vec = row_words<VC>(qc, 0) && (!dqc || row_words<VC>(dqc, 0)) && row_words<VC>(iscan, 0) &&
+                             (!qm || row_words<VC>(qm, 0)) && (!iqm || row_words<VC>(iqm, 0));
+            // the packed coefficients are one run of Wp * Hp; a word is VC of them in one row
+            auto quant = [&](auto vec_c, auto mode_c, auto qm_c) {
+                constexpr bool VEC = decltype(vec_c)::value, QM = decltype(qm_c)::value;
+                constexpr int  MODE = decltype(mode_c)::value;
+                for_words<Wp, Hp, VC, MOVERS>(tid, [&](int r, int c) {
+                    const int rc = r * Wp + c;
+                    int16_t   pos[VC];
+                    uint8_t   wt[VC], iwt[VC];
+                    int32_t   q[VC], dq[VC];
+                    ld_word<VEC>(iscan + rc, pos);
+                    if constexpr (QM) {
+                        if (qm) ld_word<VEC>(qm + rc, wt);
+                        else {
+#pragma unroll
+                            for (int j = 0; j < VC; j++) wt[j] = 1 << kQmBits;
+                        }
+                        if (iqm) ld_word<VEC>(iqm + rc, iwt);
+                        else {
+#pragma unroll
+                            for (int j = 0; j < VC; j++) iwt[j] = 1 << kQmBits;
+                        }
+                    }
+#pragma unroll
+                    for (int j = 0; j < VC; j++) {
+                        const int32_t v = fwd_out<RECT>(B[(c + j) * PH + r], cfg);
+                        quant_coef<MODE, QM>(k, v, rc + j != 0, QM ? wt[j] : 0, QM ? iwt[j] : 0, q[j], dq[j]);
+                        if (q[j]) eob = max(eob, (int)pos[j] + 1);
+                        A[(c + j) * PH + r] = inv_in<RECT>(dq[j], row_clamp);
+                    }
+                    st_word<VEC>(qc + rc, q);
+                    if (dqc) st_word<VEC>(dqc + rc, dq);
+                });
+            };
+            // the quantiser's mode and matrix once per item, then a loop specialised on them
+            with_words(vec, [&](auto vec_c) {
+                auto by_qm = [&](auto mode_c) {
+                    if (quant_has_qm(qi)) quant(vec_c, mode_c, std::true_type{});
+                    else quant(vec_c, mode_c, std::false_type{});
+                };
+                switch (qi.mode) {
+                case SVT_B200_QUANT_B_LBD: by_qm(std::integral_constant<int, SVT_B200_QUANT_B_LBD>{}); break;
+                case SVT_B200_QUANT_B_HBD: by_qm(std::integral_constant<int, SVT_B200_QUANT_B_HBD>{}); break;
+                case SVT_B200_QUANT_FP_LBD: by_qm(std::integral_constant<int, SVT_B200_QUANT_FP_LBD>{}); break;
+                default: by_qm(std::integral_constant<int, SVT_B200_QUANT_FP_HBD>{}); break;
+                }
+            });
+        } else {  // ---- Inverse: the packed dequantised coefficients are the input ----
+            const int32_t* in = g.dq_in + ii.coef_off;
+            with_words(row_words<VC>(in, 0), [&](auto vec) {
+                for_words<Wp, Hp, VC, MOVERS>(tid, [&](int r, int c) {
+                    int32_t v[VC];
+                    ld_word<decltype(vec)::value>(in + r * Wp + c, v);
+#pragma unroll
+                    for (int j = 0; j < VC; j++) A[(c + j) * PH + r] = inv_in<RECT>(v[j], row_clamp);
+                });
+            });
+        }
+        // zero outside the packed Wp x Hp
+        if constexpr (W > Wp) for_words<W - Wp, H, 1, MOVERS>(tid, [&](int r, int c) { A[(Wp + c) * PH + r] = 0; });
+        if constexpr (H > Hp) for_words<Wp, H - Hp, 1, MOVERS>(tid, [&](int r, int c) { A[c * PH + Hp + r] = 0; });
+        if constexpr (CHAIN) {
+            if constexpr (SOLO) {
+                __syncthreads();
+                if (eob) atomicMax(&s_eob, eob);
+                __syncthreads();
+                eob = s_eob;
+                if (threadIdx.x == 0) g.eobs[it] = (uint16_t)eob;
+            } else {
+                const unsigned mask = TEAM == 32 ? 0xffffffffu : (((1u << TEAM) - 1u) << ((threadIdx.x & 31) / TEAM * TEAM));
+#pragma unroll
+                for (int o = TEAM / 2; o > 0; o >>= 1) eob = max(eob, __shfl_xor_sync(mask, eob, o));
+                if (tid == 0) g.eobs[it] = (uint16_t)eob;
+                team_sync<TEAM, SOLO>();
+            }
+        } else {
+            team_sync<TEAM, SOLO>();
+        }
+        const PIX*   pr = g.pred_base + ii.pred_off;
+        PIX*         pw = g.recon_base + ii.recon_off;
+        const size_t pstride = ii.pred_stride, rstride = ii.recon_stride;
+        const bool   vec = row_words<VP>(pr, pstride) && row_words<VP>(pw, rstride);
+        if (CHAIN && eob == 0) {
+            // every level is zero: the inverse of an all-zero plane is zero, the reconstruction is the prediction
+            // (the encode pass takes the same shortcut, coding_loop.c: eob == 0 -> prediction copied); team-uniform branch
+            if (pr != pw) {
+                with_words(vec, [&](auto vec_c) {
+                    for_words<W, H, VP, MOVERS>(tid, [&](int r, int c) {
+                        PIX p[VP];
+                        ld_word<decltype(vec_c)::value>(pr + r * pstride + c, p);
+                        st_word<decltype(vec_c)::value>(pw + r * rstride + c, p);
+                    });
+                });
+            }
+            team_sync<TEAM, SOLO>();
+        } else {  // ---- inverse transform + reconstruction (inv_transforms.c:2459-2534) ----
+            const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
+            const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);  // svt_av1_gen_inv_stage_range
+            const int opt_col = bd == 12 ? 18 : 16;
+            txfm_pass<TEAM, THREADS, true, false, W, Hp, PH>(cfg.i_tr, A, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
+            team_sync<TEAM, SOLO>();
+            for_words<W, H, 1, MOVERS>(tid, [&](int r, int c) {
+                const int cs = cfg.i_lr ? (W - 1 - c) : c;
+                B[r * PW + c] = clamp_bits(round_shift_arr(A[cs * PH + r], -cfg.i_s0), col_clamp);
+            });
+            team_sync<TEAM, SOLO>();
+            txfm_pass<TEAM, THREADS, true, false, H, W, PW>(cfg.i_tc, B, cfg.i_cbc, opt_col, tid);
+            team_sync<TEAM, SOLO>();
+            const long long int_max = (1ll << (7 + bd)) - 1 + (914ll << (bd - 7));  // check_range, inv_transforms.c:2401
+            const int       pix_max = (1 << bd) - 1;
+            with_words(vec, [&](auto vec_c) {
+                for_words<W, H, VP, MOVERS>(tid, [&](int r, int c) {
+                    const int rs = cfg.i_ud ? (H - 1 - r) : r;
+                    PIX       p[VP];
+                    ld_word<decltype(vec_c)::value>(pr + r * pstride + c, p);
+#pragma unroll
+                    for (int j = 0; j < VP; j++) {
+                        long long t = (long long)round_shift_arr(B[rs * PW + c + j], -cfg.i_s1);
+                        t           = t < -int_max - 1 ? -int_max - 1 : (t > int_max ? int_max : t);
+                        int v       = (int)p[j] + (int)t;
+                        p[j]        = (PIX)(v < 0 ? 0 : (v > pix_max ? pix_max : v));
+                    }
+                    st_word<decltype(vec_c)::value>(pw + r * rstride + c, p);
+                });
+            });
+            team_sync<TEAM, SOLO>();
+        }
+    }
+}
+
+// the transform sizes of a team class (max(W,H) = TEAM), in tx_size numbers
+template <int TEAM> struct ClassSizes;
+template <> struct ClassSizes<4> { using type = std::integer_sequence<int, 0>; };
+template <> struct ClassSizes<8> { using type = std::integer_sequence<int, 1, 5, 6>; };
+template <> struct ClassSizes<16> { using type = std::integer_sequence<int, 2, 7, 8, 13, 14>; };
+template <> struct ClassSizes<32> { using type = std::integer_sequence<int, 3, 9, 10, 15, 16>; };
+template <> struct ClassSizes<64> { using type = std::integer_sequence<int, 4, 11, 12, 17, 18>; };
+
+// the item's size body, chosen once per item (team-uniform: a team runs one item)
+template <class M, int TEAM, int THREADS, typename PIX, int... SZ>
+__device__ __forceinline__ void dispatch_size(std::integer_sequence<int, SZ...>, int sz, const TxfmPtrs<PIX>& g,
+                                              const typename M::Item& item, int it, int32_t* A, int32_t* B, int tid, int& s_eob) {
+    (void)((sz == SZ && (txfm_block<M, TEAM, THREADS, PIX, SZ>(g, item, it, A, B, tid, s_eob), true)) || ...);
+}
+
+// CTAs per SM that the register allocation of a class must leave room for: what the class's kernels held before their
+// bodies were specialised by size (168 / 96 / 64 / 64 / 64 registers).  The calls of a step run concurrently on several
+// streams, so a CTA that takes more of an SM's register file keeps other kernels' CTAs off that SM; left free, ptxas
+// gives the specialised bodies up to 235 registers and the step is slower even where the class's own kernel is faster.
+template <int TEAM> constexpr int class_min_ctas() { return TEAM == 64 ? 3 : (TEAM == 32 ? 10 : (TEAM == 16 ? 8 : 4)); }
+
+template <class M, int TEAM, int THREADS, typename PIX>
+__global__ void __launch_bounds__(THREADS, class_min_ctas<TEAM>())
+txfm_kernel(const TxfmPtrs<PIX> g, const typename M::Item* __restrict__ items, int n_items) {
     extern __shared__ __align__(16) int32_t tsm[];
     // big blocks are few: one block per CTA (SOLO) of 2 * TEAM threads; all of them move its data, and lane pairs run
     // its 32- and 64-point vectors (txfm_pass)
     constexpr bool SOLO = TEAM >= 32;
-    constexpr int  TEAMS = SOLO ? 1 : THREADS / TEAM, PLANE = TEAM * (TEAM + 1), MOVERS = SOLO ? THREADS : TEAM;
+    constexpr int  TEAMS = SOLO ? 1 : THREADS / TEAM, PLANE = TEAM * (TEAM + 1);
     const int      team  = SOLO ? 0 : threadIdx.x / TEAM, tid = SOLO ? threadIdx.x : threadIdx.x % TEAM;
     int32_t*       A     = tsm + (size_t)team * team_stride(TEAM);
     int32_t*       B     = A + PLANE;
     __shared__ int s_eob;
 
-    // a Forward or Inverse item is small and is copied into registers; a Chain item is read field by field where it is used
-    using ItemRef = std::conditional_t<CHAIN, const typename M::Item&, const typename M::Item>;
+    // a Forward or Inverse item is small and is copied into registers; a Chain item is read once by its team, in 8-byte
+    // words, into shared memory, and its fields are read from there where they are used
+    using Item = typename M::Item;
+    constexpr bool STAGE = std::is_same_v<M, Chain>;
+    static_assert(sizeof(Item) % 8 == 0 && alignof(Item) == 8, "an item is whole 8-byte words");
+    __shared__ __align__(16) Item s_item[STAGE ? TEAMS : 1];
     for (int it = blockIdx.x * TEAMS + team; it < n_items; it += gridDim.x * TEAMS) {
-        const ItemRef item = items[it];
-        const auto& fi = fwd_part(item);
-        const int   sz = shape_part(item).tx_size, W = tx_w(sz), H = tx_h(sz);
-        const int   lgW = 31 - __clz(W);
-        const TxCfg cfg = c_txcfg[sz][shape_part(item).tx_type];
-        const int   rect = rect_log_ratio(W, H);
-        const int   Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;  // 64-point dimensions are packed (inv_transforms.c:2567-2686)
-        const int   PW = W + 1, PH = H + 1;  // odd pitches: a plane holds the block as [r * PW + c] or as [c * PH + r]
-        int         bd = 0;
-        if constexpr (INV) bd = inv_part(item).bd;
-        if constexpr (FWD) {  // ---- forward transform (transforms.c:2286-2318) ----
-            const int sstride = fi.src_stride;
-            // load, optional up/down flip, pre-shift
-            if constexpr (CHAIN) {
-                if (srcpix_base) {  // svt_aom_residual_kernel fused in: the source picture shares the residual plane's geometry
-                    const PIX* sp = srcpix_base + fi.src_off;
-                    const PIX* pp = pred_base + item.inv.pred_off;
-                    const int  pstride = item.inv.pred_stride;
-#pragma unroll 4
-                    for (int idx = tid; idx < W * H; idx += MOVERS) {
-                        const int r = idx >> lgW, c = idx & (W - 1);
-                        const int rr = cfg.f_ud ? (H - 1 - r) : r;
-                        const int32_t d = (int32_t)sp[(size_t)rr * sstride + c] - (int32_t)pp[(size_t)rr * pstride + c];
-                        A[r * PW + c] = round_shift_arr(d, -cfg.f_s0);
-                    }
-                }
-            }
-            if (!CHAIN || !srcpix_base) {
-                const int16_t* src = src_base + fi.src_off;
-#pragma unroll 4
-                for (int idx = tid; idx < W * H; idx += MOVERS) {
-                    const int r = idx >> lgW, c = idx & (W - 1);
-                    const int rr = cfg.f_ud ? (H - 1 - r) : r;
-                    A[r * PW + c] = round_shift_arr((int32_t)src[(size_t)rr * sstride + c], -cfg.f_s0);
-                }
-            }
+        if constexpr (STAGE) {
+            constexpr int MOVERS = SOLO ? THREADS : TEAM, WORDS = (int)(sizeof(Item) / 8);
+            for (int w = tid; w < WORDS; w += MOVERS)
+                reinterpret_cast<uint2*>(&s_item[team])[w] = reinterpret_cast<const uint2*>(items + it)[w];
             team_sync<TEAM, SOLO>();
-            // columns: vector v = column v (Chain: rows >= Hp of the result are not needed)
-            txfm_pass<TEAM, THREADS, false, !INV>(cfg.f_tc, A, H, W, PW, cfg.f_cbc, 0, tid);
-            team_sync<TEAM, SOLO>();
-            // round-shift, optional left/right flip, hand over transposed (element = column); Chain: only the Hp rows that
-            // survive the packing
-            const int Hk = INV ? Hp : H;
-#pragma unroll 4
-            for (int idx = tid; idx < W * Hk; idx += MOVERS) {
-                const int r = idx >> lgW, c = idx & (W - 1);
-                const int cc = cfg.f_lr ? (W - 1 - c) : c;
-                B[cc * PH + r] = round_shift_arr(A[r * PW + c], -cfg.f_s1);
-            }
-            team_sync<TEAM, SOLO>();
-            txfm_pass<TEAM, THREADS, false, !INV>(cfg.f_tr, B, W, Hk, PH, cfg.f_cbr, 0, tid);  // rows: vector v = row v
-            team_sync<TEAM, SOLO>();
-        }
-        if constexpr (!INV) {  // ---- Forward: the coefficients out ----
-            int32_t*  dst = coef_base + fi.dst_off;
-            const int part_shift = (fi.reserved >> 1) & 3;  // 0 full, 1 = N2, 2 = N4
-            for (int idx = tid; idx < W * H; idx += MOVERS) {
-                const int r = idx >> lgW, c = idx & (W - 1);
-                int32_t   v = fwd_out(B[c * PH + r], cfg, rect);
-                // N2 / N4 (av1_tranform_two_d_core_N2_c / _N4_c, transforms.c:5202, 6769): the top-left half / quarter
-                // of every dimension, identical to the full transform's values there, zero everywhere else
-                if (part_shift && (r >= max(H >> part_shift, 1) || c >= max(W >> part_shift, 1))) v = 0;
-                if (fi.reserved & 1) {  // packed output: keep the top-left min(W,32) x min(H,32) (svt_handle_transform64x64 repack, transforms.c:2374)
-                    if (r < Hp && c < Wp) dst[r * Wp + c] = v;
-                } else
-                    dst[idx] = v;
-            }
-            team_sync<TEAM, SOLO>();
+            const Item& item = s_item[team];  // every body ends on a team barrier: the next item's copy waits for its readers
+            dispatch_size<M, TEAM, THREADS, PIX>(typename ClassSizes<TEAM>::type{}, shape_part(item).tx_size, g, item, it, A, B, tid, s_eob);
         } else {
-            // the inverse's input plane, rows first: A[c * PH + r], element = column, vector = row; zero outside the packed
-            // Wp x Hp, which the passes keep zero
-            const auto& ii = inv_part(item);
-            const int   row_clamp = bd + 8;
-            int eob = 0;
-            if constexpr (CHAIN) {  // ---- quantise the (packed) coefficients; the dequantised levels are the input ----
-                const SvtB200QuantItem& qi = item.quant;
-                const uint8_t* qm  = qi.qm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.qm_off;
-                const uint8_t* iqm = qi.iqm_off == SVT_B200_NO_QM ? nullptr : qm_base + qi.iqm_off;
-                const int16_t* iscan = iscan_base + qi.scan_off;
-                int32_t*       qc = coef_base + qi.q_off;
-                int32_t*       dqc = dq_base ? dq_base + qi.dq_off : nullptr;
-                if (SOLO && threadIdx.x == 0) s_eob = 0;
-#pragma unroll 4
-                for (int idx = tid; idx < W * H; idx += MOVERS) {
-                    const int r = idx >> lgW, c = idx & (W - 1);
-                    int32_t   dq = 0;
-                    if (r < Hp && c < Wp) {
-                        const int32_t v = fwd_out(B[c * PH + r], cfg, rect);
-                        const int     rc = r * Wp + c;
-                        int32_t       q;
-                        quant_one(qi, v, rc, qm, iqm, q, dq);
-                        qc[rc] = q;
-                        if (dqc) dqc[rc] = dq;
-                        if (q) eob = max(eob, (int)iscan[rc] + 1);
-                        dq = inv_in(dq, rect, row_clamp);
-                    }
-                    A[c * PH + r] = dq;
-                }
-                if constexpr (SOLO) {
-                    __syncthreads();
-                    if (eob) atomicMax(&s_eob, eob);
-                    __syncthreads();
-                    eob = s_eob;
-                    if (threadIdx.x == 0) eobs[it] = (uint16_t)eob;
-                } else {
-                    const unsigned mask = TEAM == 32 ? 0xffffffffu : (((1u << TEAM) - 1u) << ((threadIdx.x & 31) / TEAM * TEAM));
-#pragma unroll
-                    for (int o = TEAM / 2; o > 0; o >>= 1) eob = max(eob, __shfl_xor_sync(mask, eob, o));
-                    if (tid == 0) eobs[it] = (uint16_t)eob;
-                    team_sync<TEAM, SOLO>();
-                }
-            } else {  // ---- Inverse: the packed dequantised coefficients are the input ----
-                const int32_t* in = dq_in + ii.coef_off;
-                for (int idx = tid; idx < W * H; idx += MOVERS) {
-                    const int r = idx >> lgW, c = idx & (W - 1);
-                    A[c * PH + r] = (r < Hp && c < Wp) ? inv_in(in[r * Wp + c], rect, row_clamp) : 0;
-                }
-                team_sync<TEAM, SOLO>();
-            }
-            if (CHAIN && eob == 0) {
-                // every level is zero: the inverse of an all-zero plane is zero, the reconstruction is the prediction
-                // (the encode pass takes the same shortcut, coding_loop.c: eob == 0 -> prediction copied); team-uniform branch
-                const PIX* pr = pred_base + ii.pred_off;
-                PIX*       pw = recon_base + ii.recon_off;
-                if (pr != pw) {
-#pragma unroll 4
-                    for (int idx = tid; idx < W * H; idx += MOVERS) {
-                        const int r = idx >> lgW, c = idx & (W - 1);
-                        pw[(size_t)r * ii.recon_stride + c] = pr[(size_t)r * ii.pred_stride + c];
-                    }
-                }
-                team_sync<TEAM, SOLO>();
-            } else {  // ---- inverse transform + reconstruction (inv_transforms.c:2459-2534) ----
-                const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
-                const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);  // svt_av1_gen_inv_stage_range
-                const int opt_col = bd == 12 ? 18 : 16;
-                txfm_pass<TEAM, THREADS, true, false>(cfg.i_tr, A, W, Hp, PH, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
-                team_sync<TEAM, SOLO>();
-#pragma unroll 4
-                for (int idx = tid; idx < W * H; idx += MOVERS) {
-                    const int r = idx >> lgW, c = idx & (W - 1);
-                    const int cs = cfg.i_lr ? (W - 1 - c) : c;
-                    B[r * PW + c] = clamp_bits(round_shift_arr(A[cs * PH + r], -cfg.i_s0), col_clamp);
-                }
-                team_sync<TEAM, SOLO>();
-                txfm_pass<TEAM, THREADS, true, false>(cfg.i_tc, B, H, W, PW, cfg.i_cbc, opt_col, tid);
-                team_sync<TEAM, SOLO>();
-                const PIX*      pr = pred_base + ii.pred_off;
-                PIX*            pw = recon_base + ii.recon_off;
-                const long long int_max = (1ll << (7 + bd)) - 1 + (914ll << (bd - 7));  // check_range, inv_transforms.c:2401
-                const int       pix_max = (1 << bd) - 1;
-#pragma unroll 4
-                for (int idx = tid; idx < W * H; idx += MOVERS) {
-                    const int r = idx >> lgW, c = idx & (W - 1);
-                    const int rs = cfg.i_ud ? (H - 1 - r) : r;
-                    long long t  = (long long)round_shift_arr(B[rs * PW + c], -cfg.i_s1);
-                    t            = t < -int_max - 1 ? -int_max - 1 : (t > int_max ? int_max : t);
-                    int p        = (int)pr[(size_t)r * ii.pred_stride + c] + (int)t;
-                    p            = p < 0 ? 0 : (p > pix_max ? pix_max : p);
-                    pw[(size_t)r * ii.recon_stride + c] = (PIX)p;
-                }
-                team_sync<TEAM, SOLO>();
-            }
+            const Item item = items[it];
+            dispatch_size<M, TEAM, THREADS, PIX>(typename ClassSizes<TEAM>::type{}, shape_part(item).tx_size, g, item, it, A, B, tid, s_eob);
         }
     }
 }
@@ -302,7 +480,7 @@ static inline int tx_class(int sz) {
 // 64-point block has its CTA of 2 * TEAM threads to itself (a lane pair per vector in the passes).
 template <int TEAM> constexpr int class_threads() { return TEAM >= 32 ? 2 * TEAM : (TEAM == 16 ? 128 : 256); }
 
-// the device buffers of a batch call, in txfm_kernel's order; each mode uses its own
+// the device buffers of a batch call as the entry points fill them, untyped; launch makes them a TxfmPtrs<PIX>
 struct TxfmBufs {
     const int16_t* residual = nullptr;
     const void*    source   = nullptr;
@@ -322,8 +500,8 @@ static void launch(const TxfmBufs& b, const typename M::Item* items, int n, uint
     constexpr size_t smem = (size_t)TEAMS * team_stride(TEAM) * 4;
     static_assert(smem <= 48 * 1024, "the default dynamic shared-memory limit: no attribute to set");
     constexpr int per_sm = (int)((200 * 1024) / (smem + 1024)) < 2048 / THREADS ? (int)((200 * 1024) / (smem + 1024)) : 2048 / THREADS;
-    txfm_kernel<M, TEAM, THREADS, PIX><<<grid_for((n + TEAMS - 1) / TEAMS, per_sm), THREADS, smem, st>>>(
-        b.residual, (const PIX*)b.source, (const PIX*)b.pred, (PIX*)b.recon, b.coef, b.dq, b.iscan, b.qm, items, n, eobs, b.dq_in);
+    const TxfmPtrs<PIX> g{b.residual, (const PIX*)b.source, (const PIX*)b.pred, (PIX*)b.recon, b.coef, b.dq, b.iscan, b.qm, eobs, b.dq_in};
+    txfm_kernel<M, TEAM, THREADS, PIX><<<grid_for((n + TEAMS - 1) / TEAMS, per_sm), THREADS, smem, st>>>(g, items, n);
     B200_LAUNCH_CHECK();
 }
 // the n items of team class cls
