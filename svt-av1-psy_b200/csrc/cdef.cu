@@ -682,25 +682,20 @@ cdef_apply_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const
 using namespace b200;
 
 // ---- T1 ------------------------------------------------------------------------------------------
-static void find_dir_t1(const uint16_t* const* imgs, int n, int stride, int coeff_shift, int* dirs, int* vars) {
+static void find_dir_t1(const uint16_t* const* imgs, int n /* 1 or 2 */, int stride, int coeff_shift, int* dirs, int* vars) {
     require_ready();
-    LaneGuard l;
+    RoundTrip rt;
     const size_t blk = 7 * (size_t)stride + 8;
-    size_t o_img = l->alloc(n * blk * 2), o_off = l->alloc(n * 4);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc(n * 8);
-    for (int i = 0; i < n; i++) {
-        memcpy(l->h<uint16_t>(o_img) + i * blk, imgs[i], blk * 2);
-        l->h<int>(o_off)[i] = (int)(i * blk);
-    }
-    l->h2d(0, in_end);
-    find_dir_kernel<<<1, 32, 0, l->stream>>>(l->d<uint16_t>(o_img), stride, coeff_shift, n, l->d<int>(o_off), l->d<int>(o_out));
+    const int off[2] = {0, (int)blk};
+    auto img = rt.in_row_list(imgs, blk, n);
+    auto o = rt.in(off, n);
+    auto out = rt.out<int>(nullptr, 2 * n);
+    find_dir_kernel<<<1, 32, 0, rt.stream()>>>(rt.dev(img), stride, coeff_shift, n, rt.dev(o), rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, n * 8);
-    l->sync();
+    rt.finish();
     for (int i = 0; i < n; i++) {
-        dirs[i] = l->h<int>(o_out)[2 * i];
-        vars[i] = l->h<int>(o_out)[2 * i + 1];
+        dirs[i] = rt.host(out)[2 * i];
+        vars[i] = rt.host(out)[2 * i + 1];
     }
 }
 
@@ -728,19 +723,15 @@ extern "C" void svt_b200_cdef_filter_block(uint8_t* dst8, uint16_t* dst16, int32
     // BlockSize: BLOCK_4X4=0, 4X8=1, 8X4=2, 8X8=3 (definitions.h:765-768)
     const int h = 4 << (bsize == 3 || bsize == 1), w = 4 << (bsize == 3 || bsize == 2);
     const int S = 144;  // CDEF_BSTRIDE (cdef.h:35)
-    LaneGuard l;
-    const int p = w + 4;
-    size_t o_in = l->alloc((size_t)p * (h + 4) * 2);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc((size_t)w * h * 2);
-    for (int r = -2; r < h + 2; r++) memcpy(l->h<uint16_t>(o_in) + (r + 2) * p, in + r * S - 2, p * 2);
-    l->h2d(0, in_end);
-    filter_block_kernel<<<1, 64, 0, l->stream>>>(l->d<uint16_t>(o_in), w, h, pri_strength, sec_strength, dir, pri_damping, sec_damping,
-                                                 coeff_shift, subsampling_factor ? subsampling_factor : 1, l->d<uint16_t>(o_out));
+    RoundTrip rt;
+    auto src = rt.in_rows(in - 2 * S - 2, S, w + 4, h + 4);  // the block and its 2-pixel border
+    auto out = rt.out<uint16_t>(nullptr, (size_t)w * h);
+    filter_block_kernel<<<1, 64, 0, rt.stream()>>>(rt.dev(src), w, h, pri_strength, sec_strength, dir, pri_damping, sec_damping,
+                                                   coeff_shift, subsampling_factor ? subsampling_factor : 1, rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, (size_t)w * h * 2);
-    l->sync();
-    const uint16_t* o = l->h<uint16_t>(o_out);
+    rt.finish();
+    // only rows i % subs == 0 are written, into whichever destination the caller passed
+    const uint16_t* o = rt.host(out);
     const int subs = subsampling_factor ? subsampling_factor : 1;
     for (int i = 0; i < h; i += subs)
         for (int j = 0; j < w; j++) {
@@ -769,21 +760,15 @@ static uint64_t cdef_dist_t1(const T* dst, int32_t dstride, const T* src, const 
         if (dlist[2 * i + 1] > maxbx) maxbx = dlist[2 * i + 1];
     }
     const size_t rows = ((size_t)maxby + 1) << bh_l2, cols = ((size_t)maxbx + 1) << bw_l2;
-    const size_t dbytes = ((rows - 1) * dstride + cols) * sizeof(T), sbytes = ((size_t)count << (bw_l2 + bh_l2)) * sizeof(T);
-    LaneGuard l;
-    size_t o_d = l->alloc(dbytes), o_s = l->alloc(sbytes), o_l = l->alloc(2 * count);
-    size_t in_end = l->used;
-    size_t o_o = l->alloc(8);
-    memcpy(l->h<uint8_t>(o_d), dst, dbytes);
-    memcpy(l->h<uint8_t>(o_s), src, sbytes);
-    memcpy(l->h<uint8_t>(o_l), dlist, 2 * count);
-    l->h2d(0, in_end);
-    cdef_dist_kernel<T><<<1, 64, 0, l->stream>>>(l->d<T>(o_d), dstride, l->d<T>(o_s), l->d<uint8_t>(o_l), count, bw_l2, bh_l2,
-                                                 coeff_shift, pli, subs ? subs : 1, l->d<unsigned long long>(o_o));
+    RoundTrip rt;
+    auto d = rt.in(dst, (rows - 1) * dstride + cols), s = rt.in(src, (size_t)count << (bw_l2 + bh_l2));
+    auto lst = rt.in(dlist, 2 * count);
+    auto out = rt.out<unsigned long long>(nullptr, 1);
+    cdef_dist_kernel<T><<<1, 64, 0, rt.stream()>>>(rt.dev(d), dstride, rt.dev(s), rt.dev(lst), count, bw_l2, bh_l2, coeff_shift, pli,
+                                                   subs ? subs : 1, rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_o, 8);
-    l->sync();
-    return *l->h<uint64_t>(o_o);
+    rt.finish();
+    return *rt.host(out);
 }
 extern "C" uint64_t svt_b200_compute_cdef_dist_16bit(const uint16_t* dst, int32_t dstride, const uint16_t* src,
                                                      const SvtB200CdefList* dlist, int32_t cdef_count, uint8_t bsize,
@@ -800,24 +785,19 @@ extern "C" uint64_t svt_b200_search_one_dual(int* lev0, int* lev1, int nb_streng
                                              int start_gi, int end_gi) {
     require_ready();
     const int ng = end_gi;
-    LaneGuard l;
-    size_t o_m0 = l->alloc((size_t)sb_count * ng * 8), o_m1 = l->alloc((size_t)sb_count * ng * 8), o_lv = l->alloc(2 * 64 * 4);
-    size_t in_end = l->used;
-    size_t o_o = l->alloc(24);
-    for (int i = 0; i < sb_count; i++) {
-        memcpy(l->h<uint64_t>(o_m0) + (size_t)i * ng, mse[0][i], (size_t)ng * 8);
-        memcpy(l->h<uint64_t>(o_m1) + (size_t)i * ng, mse[1][i], (size_t)ng * 8);
-    }
-    memcpy(l->h<int>(o_lv), lev0, nb_strengths * 4);
-    memcpy(l->h<int>(o_lv) + 64, lev1, nb_strengths * 4);
-    l->h2d(0, in_end);
-    search_one_dual_kernel<<<1, 256, (size_t)ng * ng * 8, l->stream>>>(l->d<unsigned long long>(o_m0), l->d<unsigned long long>(o_m1),
-                                                                     sb_count, ng, l->d<int>(o_lv), l->d<int>(o_lv) + 64, nb_strengths,
-                                                                     start_gi, l->d<unsigned long long>(o_o));
+    RoundTrip rt;
+    int lev[2 * 64];  // lev0 at 0, lev1 at 64
+    memcpy(lev, lev0, nb_strengths * 4);
+    memcpy(lev + 64, lev1, nb_strengths * 4);
+    auto m0 = rt.in_row_list(mse[0], ng, sb_count), m1 = rt.in_row_list(mse[1], ng, sb_count);
+    auto lv = rt.in(lev, 2 * 64);
+    auto out = rt.out<uint64_t>(nullptr, 3);
+    search_one_dual_kernel<<<1, 256, (size_t)ng * ng * 8, rt.stream()>>>((unsigned long long*)rt.dev(m0), (unsigned long long*)rt.dev(m1),
+                                                                       sb_count, ng, rt.dev(lv), rt.dev(lv) + 64, nb_strengths, start_gi,
+                                                                       (unsigned long long*)rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_o, 24);
-    l->sync();
-    const uint64_t* o = l->h<uint64_t>(o_o);
+    rt.finish();
+    const uint64_t* o = rt.host(out);
     lev0[nb_strengths] = (int)o[1];
     lev1[nb_strengths] = (int)o[2];
     return o[0];

@@ -2,11 +2,12 @@
 //
 // The library mirrors the reference's process-global dispatch model
 // (Source/Lib/Codec/aom_dsp_rtcd.c:188, common_dsp_rtcd.c:466): one global context, entry points
-// callable concurrently from any encoder worker thread.  Each host-buffer call borrows a "lane"
-// (CUDA stream + pinned staging buffer + device scratch) from a pool, stages the caller-owned host
-// memory, launches, and copies results back before returning -- the reference contract is that
-// outputs are fully written on return (SURVEY.md 8b).  There is NO CPU fallback: if the device is
-// missing the entry points abort.
+// callable concurrently from any encoder worker thread.  Each host-buffer call is one RoundTrip: it
+// borrows a "lane" (CUDA stream + pinned staging buffer + device buffer of the same layout) from a
+// pool, declares the caller memory it sends and the memory it gets back, launches, and has the
+// results written back before it returns -- the reference contract is that outputs are fully
+// written on return (SURVEY.md 8b).  There is NO CPU fallback: if the device is missing the entry
+// points abort.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -31,28 +32,12 @@ namespace b200 {
 struct Lane {
     cudaStream_t stream   = nullptr;
     uint8_t*     h_buf    = nullptr;  // pinned host staging
-    uint8_t*     d_buf    = nullptr;  // device scratch, same layout as h_buf
+    uint8_t*     d_buf    = nullptr;  // device buffer, same layout as h_buf
     size_t       cap      = 0;
-    size_t       used     = 0;
     bool         busy     = false;
 
+    // grow both buffers to at least `bytes`; what they held is not kept
     void reserve(size_t bytes);
-    // bump-allocate `bytes` (256-B aligned) in both buffers; returns the offset
-    size_t alloc(size_t bytes) {
-        size_t off = (used + 255) & ~size_t(255);
-        reserve(off + bytes + 256);
-        used = off + bytes;
-        return off;
-    }
-    template <typename T> T* h(size_t off) { return reinterpret_cast<T*>(h_buf + off); }
-    template <typename T> T* d(size_t off) { return reinterpret_cast<T*>(d_buf + off); }
-    void h2d(size_t off, size_t bytes) {
-        if (bytes) B200_CUDA_CHECK(cudaMemcpyAsync(d_buf + off, h_buf + off, bytes, cudaMemcpyHostToDevice, stream));
-    }
-    void d2h(size_t off, size_t bytes) {
-        if (bytes) B200_CUDA_CHECK(cudaMemcpyAsync(h_buf + off, d_buf + off, bytes, cudaMemcpyDeviceToHost, stream));
-    }
-    void sync() { B200_CUDA_CHECK(cudaStreamSynchronize(stream)); }
 };
 
 struct Context {
@@ -66,7 +51,6 @@ struct Context {
     // lifetime of module state (svt_b200_shutdown -> svt_b200_init on another device must not meet anything of the old one)
     int                          epoch = 0;      // bumped by every successful svt_b200_init
     std::vector<void*>           scratch;        // every device scratch buffer of every module: freed at shutdown, never earlier
-    std::vector<void (*)()>      resets;         // per-module "forget your cached pointers" hooks
     std::vector<cudaStream_t>    side_streams;   // ForkJoin handles of all host threads
     std::vector<cudaEvent_t>     side_events;
 };
@@ -96,17 +80,87 @@ struct ForkJoin {
 ForkJoin& fork_streams(cudaStream_t user);
 void      join_streams(ForkJoin& fj, cudaStream_t user);
 
-struct LaneGuard {
-    Lane* l;
-    LaneGuard() : l(lane_acquire()) {}
-    ~LaneGuard() { lane_release(l); }
-    Lane* operator->() { return l; }
-};
+// One synchronous host round trip of a T1 (or `_batch_host`) call on a lane.  The call declares regions, launches on
+// stream() with dev() pointers, and calls finish().  The first fill() or dev() seals the layout: inputs, then in-outs,
+// then outputs, then device-only scratch, each 256-B aligned, with 256 B of slack after the last (kernels may read a
+// little past a region); it sizes the lane once and packs the declared inputs.  The first dev() sends inputs and
+// in-outs with one copy.  finish() fetches in-outs and outputs with one copy, synchronises, and writes back exactly the
+// declared destinations; a call that writes back less than it fetched reads host() after finish() and unpacks by hand.
+// Pitches and sizes count elements of T.  A null source leaves a region unpacked; a null destination is not written.
+class RoundTrip {
+  public:
+    template <typename T> struct Buf { int i; };
 
-// copy a strided 2-D host region into a packed staging area
-static inline void copy2d(uint8_t* dst, size_t dpitch, const uint8_t* src, size_t spitch, size_t wbytes, size_t rows) {
-    for (size_t r = 0; r < rows; r++) memcpy(dst + r * dpitch, src + r * spitch, wbytes);
-}
+    RoundTrip() : l_(lane_acquire()) {}
+    ~RoundTrip() { lane_release(l_); }
+    RoundTrip(const RoundTrip&)            = delete;
+    RoundTrip& operator=(const RoundTrip&) = delete;
+
+    // `n_alloc` (> n) sizes a region that must be larger than its data, e.g. for a kernel that reads past it
+    template <typename T> Buf<T> in(const T* p, size_t n, size_t n_alloc = 0) {
+        return {add(kIn, sizeof(T), n, 1, n_alloc, p, nullptr, n, nullptr, 0)};
+    }
+    // rows of w elements, packed at pitch w
+    template <typename T> Buf<T> in_rows(const T* p, size_t pitch, size_t w, size_t rows) {
+        return {add(kIn, sizeof(T), w, rows, 0, p, nullptr, pitch, nullptr, 0)};
+    }
+    // one row pointer per row (a null row is left unpacked), packed at pitch w
+    template <typename T> Buf<T> in_row_list(const T* const* row, size_t w, size_t rows, size_t n_alloc = 0) {
+        return {add(kIn, sizeof(T), w, rows, n_alloc, nullptr, reinterpret_cast<const void* const*>(row), 0, nullptr, 0)};
+    }
+    template <typename T> Buf<T> inout(T* p, size_t n) { return {add(kInOut, sizeof(T), n, 1, 0, p, nullptr, n, p, n)}; }
+    template <typename T> Buf<T> out(T* dst, size_t n, size_t n_alloc = 0) {
+        return {add(kOut, sizeof(T), n, 1, n_alloc, nullptr, nullptr, 0, dst, n)};
+    }
+    template <typename T> Buf<T> out_rows(T* dst, size_t pitch, size_t w, size_t rows) {
+        return {add(kOut, sizeof(T), w, rows, 0, nullptr, nullptr, 0, dst, pitch)};
+    }
+    template <typename T> Buf<T> scratch(size_t n) { return {add(kScratch, sizeof(T), n, 1, 0, nullptr, nullptr, 0, nullptr, 0)}; }
+
+    // host view of an input region, to pack by hand what no declaration describes; only before the first dev()
+    template <typename T> T* fill(Buf<T> b) {
+        if (state_ == kOpen) seal();
+        if (state_ != kSealed || slot_[b.i].kind != kIn) misuse("fill() of a region that is not an unsent input");
+        return reinterpret_cast<T*>(l_->h_buf + slot_[b.i].off);
+    }
+    template <typename T> T* dev(Buf<T> b) {
+        if (state_ != kSent) send();
+        return reinterpret_cast<T*>(l_->d_buf + slot_[b.i].off);
+    }
+    cudaStream_t stream() const { return l_->stream; }
+    void         finish();
+    template <typename T> T* host(Buf<T> b) {
+        if (state_ != kDone) misuse("host() before finish()");
+        return reinterpret_cast<T*>(l_->h_buf + slot_[b.i].off);
+    }
+
+  private:
+    enum Kind : uint8_t { kIn, kInOut, kOut, kScratch };
+    enum State : uint8_t { kOpen, kSealed, kSent, kDone };
+    struct Slot {
+        Kind               kind;
+        size_t             bytes, off;       // the region
+        size_t             row_bytes, rows;  // what is packed into it / written back from it, at pitch row_bytes
+        const uint8_t*     src;              // packed from rows at src_pitch ...
+        const void* const* src_row;          // ... or from one pointer per row
+        size_t             src_pitch;
+        uint8_t*           dst;              // written back to rows at dst_pitch
+        size_t             dst_pitch;
+    };
+    static constexpr int kSlots = 8;
+
+    int  add(Kind kind, size_t elem, size_t w, size_t rows, size_t n_alloc, const void* src, const void* const* src_row,
+             size_t src_pitch, void* dst, size_t dst_pitch);
+    void seal();
+    void send();
+    [[noreturn]] static void misuse(const char* what);
+
+    Lane*  l_;
+    Slot   slot_[kSlots];
+    int    n_     = 0;
+    State  state_ = kOpen;
+    size_t h2d_bytes_ = 0, d2h_off_ = 0, d2h_bytes_ = 0;
+};
 
 static inline int grid_for(long long work_ctas, int ctas_per_sm = 8) {
     long long cap = (long long)ctx().sm_count * ctas_per_sm;

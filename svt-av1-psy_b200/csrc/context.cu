@@ -7,25 +7,94 @@ namespace b200 {
 static Context g_ctx;
 Context& ctx() { return g_ctx; }
 
+// A round trip sizes its lane once, before it packs anything, and every round trip synchronises before it releases the
+// lane: the old buffers hold nothing and nothing is in flight on them.
 void Lane::reserve(size_t bytes) {
     if (bytes <= cap) return;
     size_t ncap = cap ? cap : (size_t(4) << 20);
     while (ncap < bytes) ncap *= 2;
-    uint8_t* nh = nullptr;
-    uint8_t* nd = nullptr;
-    B200_CUDA_CHECK(cudaHostAlloc(&nh, ncap, cudaHostAllocDefault));
-    B200_CUDA_CHECK(cudaMalloc(&nd, ncap));
     if (h_buf) {
-        // growing in the middle of a call: preserve what was staged so far
-        B200_CUDA_CHECK(cudaStreamSynchronize(stream));
-        memcpy(nh, h_buf, used);
-        B200_CUDA_CHECK(cudaMemcpy(nd, d_buf, used, cudaMemcpyDeviceToDevice));
         B200_CUDA_CHECK(cudaFreeHost(h_buf));
         B200_CUDA_CHECK(cudaFree(d_buf));
     }
-    h_buf = nh;
-    d_buf = nd;
-    cap   = ncap;
+    B200_CUDA_CHECK(cudaHostAlloc(&h_buf, ncap, cudaHostAllocDefault));
+    B200_CUDA_CHECK(cudaMalloc(&d_buf, ncap));
+    cap = ncap;
+}
+
+static void copy2d(uint8_t* dst, size_t dpitch, const uint8_t* src, size_t spitch, size_t wbytes, size_t rows) {
+    for (size_t r = 0; r < rows; r++) memcpy(dst + r * dpitch, src + r * spitch, wbytes);
+}
+
+void RoundTrip::misuse(const char* what) {
+    fprintf(stderr, "[svt_b200] FATAL: round trip: %s\n", what);
+    abort();
+}
+
+int RoundTrip::add(Kind kind, size_t elem, size_t w, size_t rows, size_t n_alloc, const void* src, const void* const* src_row,
+                   size_t src_pitch, void* dst, size_t dst_pitch) {
+    if (state_ != kOpen) misuse("region declared after the layout was sealed");
+    if (n_ == kSlots) misuse("more regions than the slot table holds");
+    Slot& s     = slot_[n_];
+    s.kind      = kind;
+    s.row_bytes = w * elem;
+    s.rows      = rows;
+    s.bytes     = n_alloc > w * rows ? n_alloc * elem : s.row_bytes * rows;
+    s.src       = static_cast<const uint8_t*>(src);
+    s.src_row   = src_row;
+    s.src_pitch = src_pitch * elem;
+    s.dst       = static_cast<uint8_t*>(dst);
+    s.dst_pitch = dst_pitch * elem;
+    return n_++;
+}
+
+void RoundTrip::seal() {
+    size_t end = 0, d2h_off = ~size_t(0);
+    for (int k = kIn; k <= kScratch; k++) {
+        for (int i = 0; i < n_; i++) {
+            Slot& s = slot_[i];
+            if (s.kind != k) continue;
+            s.off = (end + 255) & ~size_t(255);
+            end   = s.off + s.bytes;
+            if ((k == kInOut || k == kOut) && d2h_off == ~size_t(0)) d2h_off = s.off;
+        }
+        if (k == kInOut) h2d_bytes_ = end;
+        if (k == kOut && d2h_off != ~size_t(0)) {
+            d2h_off_   = d2h_off;
+            d2h_bytes_ = end - d2h_off;
+        }
+    }
+    l_->reserve(end + 256);
+    for (int i = 0; i < n_; i++) {
+        const Slot& s = slot_[i];
+        uint8_t*    h = l_->h_buf + s.off;
+        if (s.src_row) {
+            for (size_t r = 0; r < s.rows; r++)
+                if (s.src_row[r]) memcpy(h + r * s.row_bytes, s.src_row[r], s.row_bytes);
+        } else if (s.src) {
+            copy2d(h, s.row_bytes, s.src, s.src_pitch, s.row_bytes, s.rows);
+        }
+    }
+    state_ = kSealed;
+}
+
+void RoundTrip::send() {
+    if (state_ == kDone) misuse("dev() after finish()");
+    if (state_ == kOpen) seal();
+    if (h2d_bytes_) B200_CUDA_CHECK(cudaMemcpyAsync(l_->d_buf, l_->h_buf, h2d_bytes_, cudaMemcpyHostToDevice, l_->stream));
+    state_ = kSent;
+}
+
+void RoundTrip::finish() {
+    if (state_ != kSent) send();
+    if (d2h_bytes_)
+        B200_CUDA_CHECK(cudaMemcpyAsync(l_->h_buf + d2h_off_, l_->d_buf + d2h_off_, d2h_bytes_, cudaMemcpyDeviceToHost, l_->stream));
+    B200_CUDA_CHECK(cudaStreamSynchronize(l_->stream));
+    for (int i = 0; i < n_; i++) {
+        const Slot& s = slot_[i];
+        if (s.dst) copy2d(s.dst, s.dst_pitch, l_->h_buf + s.off, s.row_bytes, s.row_bytes, s.rows);
+    }
+    state_ = kDone;
 }
 
 void require_ready() {
@@ -46,7 +115,6 @@ Lane* lane_acquire() {
     for (Lane* l : g_ctx.lanes)
         if (!l->busy) {
             l->busy = true;
-            l->used = 0;
             B200_CUDA_CHECK(cudaSetDevice(g_ctx.device));
             return l;
         }
@@ -129,7 +197,6 @@ extern "C" void svt_b200_shutdown(void) {
         std::lock_guard<std::mutex> rl(reset_mu());
         for (void (*fn)() : reset_list()) fn();   // modules forget their cached scratch / per-stream state ...
     }
-    if (false) for (void (*fn)() : c.resets) fn();           // modules forget their cached scratch / per-stream state ...
     for (void* p : c.scratch) cudaFree(p);        // ... and the scratch itself goes (nothing was freed before: captured graphs)
     c.scratch.clear();
     for (cudaStream_t s : c.side_streams) cudaStreamDestroy(s);

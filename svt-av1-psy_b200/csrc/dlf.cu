@@ -224,20 +224,17 @@ template <int TAPS, typename T>
 static void lpf_t1(T* s, int32_t pitch, const uint8_t* blimit, const uint8_t* limit, const uint8_t* thresh, int bd, bool vertical) {
     require_ready();
     constexpr int D = Depth<TAPS>::read, W = Depth<TAPS>::write;
-    const size_t bytes = 4 * 2 * D * sizeof(T);
-    LaneGuard l;
-    const size_t o = l->alloc(bytes);
-    T* h = l->h<T>(o);
+    RoundTrip rt;
+    T px[4 * 2 * D];  // D pixels either side of the edge on each of the 4 lines; W of them are written back
     const ptrdiff_t across = vertical ? 1 : pitch, along = vertical ? pitch : 1;
     for (int i = 0; i < 4; i++)
-        for (int k = -D; k < D; k++) h[i * 2 * D + D + k] = s[i * along + k * across];
-    l->h2d(o, bytes);
-    lpf_t1_kernel<TAPS, T><<<1, 32, 0, l->stream>>>(l->d<T>(o), *blimit, *limit, *thresh, bd - 8);
+        for (int k = -D; k < D; k++) px[i * 2 * D + D + k] = s[i * along + k * across];
+    auto b = rt.inout(px, 4 * 2 * D);
+    lpf_t1_kernel<TAPS, T><<<1, 32, 0, rt.stream()>>>(rt.dev(b), *blimit, *limit, *thresh, bd - 8);
     B200_LAUNCH_CHECK();
-    l->d2h(o, bytes);
-    l->sync();
+    rt.finish();
     for (int i = 0; i < 4; i++)
-        for (int k = -W; k < W; k++) s[i * along + k * across] = h[i * 2 * D + D + k];
+        for (int k = -W; k < W; k++) s[i * along + k * across] = px[i * 2 * D + D + k];
 }
 
 #define B200_DEF_LPF(DIR, N, VERT)                                                                                            \

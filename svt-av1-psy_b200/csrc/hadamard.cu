@@ -149,21 +149,16 @@ __global__ void satd_kernel(const int32_t* __restrict__ coeff, int length, int32
 
 static void hadamard_t1(const int16_t* src_diff, ptrdiff_t src_stride, int32_t* coeff, int n) {
     require_ready();
-    LaneGuard l;
-    size_t o_src = l->alloc((size_t)n * n * 2), o_it = l->alloc(sizeof(SvtB200HadamardItem));
-    size_t in_end = l->used;
-    size_t o_c = l->alloc((size_t)n * n * 4);
-    for (int r = 0; r < n; r++) memcpy(l->h<int16_t>(o_src) + r * n, src_diff + (ptrdiff_t)r * src_stride, n * 2);
-    SvtB200HadamardItem* it = l->h<SvtB200HadamardItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->src_stride = n;
-    it->size = n;
-    l->h2d(0, in_end);
-    hadamard_kernel<<<1, 128, 0, l->stream>>>(l->d<int16_t>(o_src), l->d<SvtB200HadamardItem>(o_it), 1, l->d<int32_t>(o_c), nullptr);
+    RoundTrip rt;
+    SvtB200HadamardItem item{};
+    item.src_stride = n;
+    item.size = n;
+    auto src = rt.in_rows(src_diff, src_stride, n, n);
+    auto it = rt.in(&item, 1);
+    auto c = rt.out(coeff, (size_t)n * n);
+    hadamard_kernel<<<1, 128, 0, rt.stream()>>>(rt.dev(src), rt.dev(it), 1, rt.dev(c), nullptr);
     B200_LAUNCH_CHECK();
-    l->d2h(o_c, (size_t)n * n * 4);
-    l->sync();
-    memcpy(coeff, l->h<int32_t>(o_c), (size_t)n * n * 4);
+    rt.finish();
 }
 
 // ---- hadamard_path (enc_mode_config.c:2147-2212): residual -> Hadamard -> SATD of every transform block of a prediction block ----
@@ -257,43 +252,30 @@ extern "C" uint32_t svt_b200_hadamard_path(SvtB200Buf2D residual, SvtB200Buf2D c
     const int n = maxtx[bsize] > 32 ? 32 : maxtx[bsize];  // AOMMIN(TX_32X32, max_txsize_lookup[bsize])
     const int side = wide[bsize];                          // the reference walks block_size_wide in BOTH directions
     const int per_row = side / n, nblk = per_row * per_row;
-    LaneGuard l;
-    size_t o_in = l->alloc((size_t)side * side), o_pr = l->alloc((size_t)side * side);
-    size_t in_end = l->used;
-    size_t o_satd = l->alloc((size_t)nblk * 4), o_res = l->alloc((size_t)n * n * 2), o_co = l->alloc((size_t)n * n * 4);
-    for (int r = 0; r < side; r++) {
-        memcpy(l->h<uint8_t>(o_in) + (size_t)r * side, input.buf + (size_t)r * input.stride, side);
-        memcpy(l->h<uint8_t>(o_pr) + (size_t)r * side, pred.buf + (size_t)r * pred.stride, side);
-    }
-    l->h2d(0, in_end);
-    HadPathArgs a = {l->d<uint8_t>(o_in), l->d<uint8_t>(o_pr), side, side, n, per_row, nblk};
-    hadamard_path_kernel<<<nblk, 128, 0, l->stream>>>(a, l->d<int32_t>(o_satd), l->d<int16_t>(o_res), l->d<int32_t>(o_co));
-    B200_LAUNCH_CHECK();
-    l->d2h(o_satd, (o_co + (size_t)n * n * 4) - o_satd);
-    l->sync();
-    uint32_t cost = 0;
-    for (int i = 0; i < nblk; i++) cost += (uint32_t)l->h<int32_t>(o_satd)[i];
+    RoundTrip rt;
+    auto in = rt.in_rows(input.buf, input.stride, side, side), pr = rt.in_rows(pred.buf, pred.stride, side, side);
+    auto satd = rt.out<int32_t>(nullptr, nblk);
     // the loop of the reference leaves the LAST block's residual (at its stride) and coefficients in the caller's buffers
-    int16_t* rb = reinterpret_cast<int16_t*>(residual.buf);
-    for (int r = 0; r < n; r++) memcpy(rb + (size_t)r * residual.stride, l->h<int16_t>(o_res) + (size_t)r * n, (size_t)n * 2);
-    memcpy(coeff.buf, l->h<int32_t>(o_co), (size_t)n * n * 4);
+    auto res = rt.out_rows(reinterpret_cast<int16_t*>(residual.buf), residual.stride, n, n);
+    auto co = rt.out(reinterpret_cast<int32_t*>(coeff.buf), (size_t)n * n);
+    HadPathArgs a = {rt.dev(in), rt.dev(pr), side, side, n, per_row, nblk};
+    hadamard_path_kernel<<<nblk, 128, 0, rt.stream()>>>(a, rt.dev(satd), rt.dev(res), rt.dev(co));
+    B200_LAUNCH_CHECK();
+    rt.finish();
+    uint32_t cost = 0;
+    for (int i = 0; i < nblk; i++) cost += (uint32_t)rt.host(satd)[i];
     return cost;
 }
 
 // T1: svt_av1_fwht4x4 (aom_dsp_rtcd.h:208)
 extern "C" void svt_b200_av1_fwht4x4(int16_t* input, int32_t* output, uint32_t stride) {
     require_ready();
-    LaneGuard l;
-    size_t o_in = l->alloc(32);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc(64);
-    for (int r = 0; r < 4; r++) memcpy(l->h<int16_t>(o_in) + 4 * r, input + (size_t)r * stride, 8);
-    l->h2d(0, in_end);
-    fwht4x4_kernel<<<1, 32, 0, l->stream>>>(l->d<int16_t>(o_in), l->d<int32_t>(o_out));
+    RoundTrip rt;
+    auto in = rt.in_rows(input, stride, 4, 4);
+    auto out = rt.out(output, 16);
+    fwht4x4_kernel<<<1, 32, 0, rt.stream()>>>(rt.dev(in), rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, 64);
-    l->sync();
-    memcpy(output, l->h<int32_t>(o_out), 64);
+    rt.finish();
 }
 
 // T1: svt_av1_compute_cul_level (aom_dsp_rtcd.h:904)
@@ -302,18 +284,14 @@ extern "C" uint8_t svt_b200_av1_compute_cul_level(const int16_t* const scan, con
     const int n = *eob;
     int maxpos = 0;
     for (int c = 0; c < n; c++) maxpos = scan[c] > maxpos ? scan[c] : maxpos;
-    LaneGuard l;
-    size_t o_sc = l->alloc((size_t)(n > 0 ? n : 1) * 2), o_q = l->alloc((size_t)(maxpos + 1) * 4);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc(16);
-    if (n) memcpy(l->h<int16_t>(o_sc), scan, (size_t)n * 2);
-    memcpy(l->h<int32_t>(o_q), quant_coeff, (size_t)(maxpos + 1) * 4);
-    l->h2d(0, in_end);
-    cul_level_kernel<<<1, 128, 0, l->stream>>>(l->d<int16_t>(o_sc), l->d<int32_t>(o_q), n, l->d<int32_t>(o_out));
+    RoundTrip rt;
+    auto sc = rt.in(scan, n, 1);
+    auto q = rt.in(quant_coeff, maxpos + 1);
+    auto out = rt.out<int32_t>(nullptr, 4);
+    cul_level_kernel<<<1, 128, 0, rt.stream()>>>(rt.dev(sc), rt.dev(q), n, rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, 4);
-    l->sync();
-    return (uint8_t)*l->h<int32_t>(o_out);
+    rt.finish();
+    return (uint8_t)*rt.host(out);
 }
 
 extern "C" void svt_b200_aom_hadamard_4x4(const int16_t* src_diff, ptrdiff_t src_stride, int32_t* coeff) { hadamard_t1(src_diff, src_stride, coeff, 4); }
@@ -324,17 +302,13 @@ extern "C" void svt_b200_aom_hadamard_32x32(const int16_t* src_diff, ptrdiff_t s
 extern "C" int svt_b200_aom_satd(const int32_t* coeff, int length) {
     require_ready();
     if (length <= 0) return 0;
-    LaneGuard l;
-    size_t o_c = l->alloc((size_t)length * 4);
-    size_t in_end = l->used;
-    size_t o_o = l->alloc(16);
-    memcpy(l->h<int32_t>(o_c), coeff, (size_t)length * 4);
-    l->h2d(0, in_end);
-    satd_kernel<<<1, 256, 0, l->stream>>>(l->d<int32_t>(o_c), length, l->d<int32_t>(o_o));
+    RoundTrip rt;
+    auto c = rt.in(coeff, length);
+    auto out = rt.out<int32_t>(nullptr, 4);
+    satd_kernel<<<1, 256, 0, rt.stream()>>>(rt.dev(c), length, rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_o, 4);
-    l->sync();
-    return *l->h<int32_t>(o_o);
+    rt.finish();
+    return *rt.host(out);
 }
 
 extern "C" int svt_b200_hadamard_satd_batch_dev(const int16_t* d_residual, const SvtB200HadamardItem* d_items, int n_items,

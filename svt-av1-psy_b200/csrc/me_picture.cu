@@ -60,18 +60,13 @@ extern "C" void svt_b200_downsample_2d(uint8_t* input_samples, uint32_t input_st
     const uint32_t half = decim_step >> 1;
     if (input_area_width <= half || input_area_height <= half) return;
     const uint32_t ow = (input_area_width - half + decim_step - 1) / decim_step, oh = (input_area_height - half + decim_step - 1) / decim_step;
-    LaneGuard l;
-    size_t o_in = l->alloc((size_t)input_area_height * input_area_width);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc((size_t)ow * oh);
-    for (uint32_t r = 0; r < input_area_height; r++) memcpy(l->h<uint8_t>(o_in) + (size_t)r * input_area_width, input_samples + (size_t)r * input_stride, input_area_width);
-    l->h2d(0, in_end);
-    downsample_2d_kernel<<<grid_for((ow * oh + 255) / 256, 8), 256, 0, l->stream>>>(l->d<uint8_t>(o_in), (int)input_area_width, (int)input_area_width,
-                                                                                 (int)input_area_height, l->d<uint8_t>(o_out), (int)ow, (int)decim_step);
+    RoundTrip rt;
+    auto in = rt.in_rows(input_samples, input_stride, input_area_width, input_area_height);
+    auto out = rt.out_rows(decim_samples, decim_stride, ow, oh);
+    downsample_2d_kernel<<<grid_for((ow * oh + 255) / 256, 8), 256, 0, rt.stream()>>>(rt.dev(in), (int)input_area_width, (int)input_area_width,
+                                                                                   (int)input_area_height, rt.dev(out), (int)ow, (int)decim_step);
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, (size_t)ow * oh);
-    l->sync();
-    for (uint32_t r = 0; r < oh; r++) memcpy(decim_samples + (size_t)r * decim_stride, l->h<uint8_t>(o_out) + (size_t)r * ow, ow);
+    rt.finish();
 }
 
 struct PadPlanes {

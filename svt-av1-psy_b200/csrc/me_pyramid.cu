@@ -426,57 +426,46 @@ extern "C" void svt_b200_ext_all_sad_calculation_8x8_16x16(uint8_t* src, uint32_
                                                            uint8_t sub_sad) {
     (void)p_eight_sad8x8;  // not written by the reference C kernel either (motion_estimation.c:221)
     require_ready();
-    LaneGuard l;
+    RoundTrip rt;
     const size_t sb = 63 * (size_t)src_stride + 64, rb = 63 * (size_t)ref_stride + 64 + 7;
-    size_t o_src = l->alloc(sb), o_ref = l->alloc(rb);
-    size_t o_st = l->alloc((64 + 16 + 64 + 16) * 4);  // best8, best16, mv8, mv16
-    size_t in_end = l->used;
-    size_t o_e16 = l->alloc(16 * 8 * 4);
-    memcpy(l->h<uint8_t>(o_src), src, sb);
-    memcpy(l->h<uint8_t>(o_ref), ref, rb);
-    uint32_t* st = l->h<uint32_t>(o_st);
+    uint32_t st[64 + 16 + 64 + 16];  // best8, best16, mv8, mv16
     memcpy(st, p_best_sad_8x8, 64 * 4);
     memcpy(st + 64, p_best_sad_16x16, 16 * 4);
     memcpy(st + 80, p_best_mv8x8, 64 * 4);
     memcpy(st + 144, p_best_mv16x16, 16 * 4);
-    l->h2d(0, in_end);
-    uint32_t* d = l->d<uint32_t>(o_st);
-    ext_all_sad_kernel<<<1, 64, 0, l->stream>>>(l->d<uint8_t>(o_src), src_stride, l->d<uint8_t>(o_ref), ref_stride, mv, d, d + 64,
-                                                d + 80, d + 144, l->d<uint32_t>(o_e16), sub_sad ? 1 : 0);
+    auto s = rt.in(src, sb), r = rt.in(ref, rb);
+    auto best = rt.inout(st, 64 + 16 + 64 + 16);
+    auto e16 = rt.out(&p_eight_sad16x16[0][0], 16 * 8);
+    uint32_t* d = rt.dev(best);
+    ext_all_sad_kernel<<<1, 64, 0, rt.stream()>>>(rt.dev(s), src_stride, rt.dev(r), ref_stride, mv, d, d + 64, d + 80, d + 144,
+                                                  rt.dev(e16), sub_sad ? 1 : 0);
     B200_LAUNCH_CHECK();
-    l->d2h(o_st, (o_e16 + 16 * 8 * 4) - o_st);
-    l->sync();
+    rt.finish();
     memcpy(p_best_sad_8x8, st, 64 * 4);
     memcpy(p_best_sad_16x16, st + 64, 16 * 4);
     memcpy(p_best_mv8x8, st + 80, 64 * 4);
     memcpy(p_best_mv16x16, st + 144, 16 * 4);
-    memcpy(p_eight_sad16x16, l->h<uint32_t>(o_e16), 16 * 8 * 4);
 }
 
 static void ext_32_64_t1(const uint32_t* sad16, uint32_t* b32, uint32_t* b64, uint32_t* m32, uint32_t* m64, uint32_t mv,
                          uint32_t* sad32, int n_idx) {
     require_ready();
-    LaneGuard l;
-    size_t o_in = l->alloc(16 * 8 * 4), o_st = l->alloc(10 * 4);
-    size_t in_end = l->used;
-    size_t o_s32 = l->alloc(4 * 8 * 4);
-    memcpy(l->h<uint32_t>(o_in), sad16, (size_t)16 * n_idx * 4);
-    uint32_t* st = l->h<uint32_t>(o_st);
+    RoundTrip rt;
+    uint32_t st[10];
     memcpy(st, b32, 16);
     st[4] = b64[0];
     memcpy(st + 5, m32, 16);
     st[9] = m64[0];
-    l->h2d(0, in_end);
-    uint32_t* d = l->d<uint32_t>(o_st);
-    ext_sad_32_64_kernel<<<1, 32, 0, l->stream>>>(l->d<uint32_t>(o_in), d, d + 4, d + 5, d + 9, mv, l->d<uint32_t>(o_s32), n_idx);
+    auto in = rt.in(sad16, (size_t)16 * n_idx, 16 * 8), best = rt.inout(st, 10);
+    auto s32 = rt.out(sad32, (size_t)4 * n_idx, 4 * 8);
+    uint32_t* d = rt.dev(best);
+    ext_sad_32_64_kernel<<<1, 32, 0, rt.stream()>>>(rt.dev(in), d, d + 4, d + 5, d + 9, mv, rt.dev(s32), n_idx);
     B200_LAUNCH_CHECK();
-    l->d2h(o_st, (o_s32 + 4 * 8 * 4) - o_st);
-    l->sync();
+    rt.finish();
     memcpy(b32, st, 16);
     b64[0] = st[4];
     memcpy(m32, st + 5, 16);
     m64[0] = st[9];
-    memcpy(sad32, l->h<uint32_t>(o_s32), (size_t)4 * n_idx * 4);
 }
 
 extern "C" void svt_b200_ext_eight_sad_calculation_32x32_64x64(uint32_t p_sad16x16[16][8], uint32_t* p_best_sad_32x32,
@@ -495,32 +484,26 @@ extern "C" void svt_b200_ext_sad_calculation_8x8_16x16(uint8_t* src, uint32_t sr
                                                        uint32_t* p_best_mv16x16, uint32_t mv, uint32_t* p_sad16x16,
                                                        uint32_t* p_sad8x8, uint8_t sub_sad) {
     require_ready();
-    LaneGuard l;
+    RoundTrip rt;
     const size_t sb = 15 * (size_t)src_stride + 16, rb = 15 * (size_t)ref_stride + 16;
-    size_t o_src = l->alloc(sb), o_ref = l->alloc(rb), o_st = l->alloc(10 * 4);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc(5 * 4);
-    memcpy(l->h<uint8_t>(o_src), src, sb);
-    memcpy(l->h<uint8_t>(o_ref), ref, rb);
-    uint32_t* st = l->h<uint32_t>(o_st);
+    uint32_t st[10];
     memcpy(st, p_best_sad_8x8, 16);
     st[4] = p_best_sad_16x16[0];
     memcpy(st + 5, p_best_mv8x8, 16);
     st[9] = p_best_mv16x16[0];
-    l->h2d(0, in_end);
-    uint32_t* d = l->d<uint32_t>(o_st);
-    uint32_t* o = l->d<uint32_t>(o_out);
-    ext_sad_8_16_kernel<<<1, 4, 0, l->stream>>>(l->d<uint8_t>(o_src), src_stride, l->d<uint8_t>(o_ref), ref_stride, d, d + 4, d + 5,
-                                                d + 9, mv, o + 4, o, sub_sad ? 1 : 0);
+    auto s = rt.in(src, sb), r = rt.in(ref, rb);
+    auto best = rt.inout(st, 10);
+    auto sad = rt.out(p_sad8x8, 4, 5);  // the four 8x8 SADs, then the 16x16 one
+    uint32_t *d = rt.dev(best), *o = rt.dev(sad);
+    ext_sad_8_16_kernel<<<1, 4, 0, rt.stream()>>>(rt.dev(s), src_stride, rt.dev(r), ref_stride, d, d + 4, d + 5, d + 9, mv, o + 4, o,
+                                                  sub_sad ? 1 : 0);
     B200_LAUNCH_CHECK();
-    l->d2h(o_st, (o_out + 20) - o_st);
-    l->sync();
+    rt.finish();
     memcpy(p_best_sad_8x8, st, 16);
     p_best_sad_16x16[0] = st[4];
     memcpy(p_best_mv8x8, st + 5, 16);
     p_best_mv16x16[0] = st[9];
-    memcpy(p_sad8x8, l->h<uint32_t>(o_out), 16);
-    *p_sad16x16 = l->h<uint32_t>(o_out)[4];
+    *p_sad16x16 = rt.host(sad)[4];
 }
 
 // svt_initialize_buffer_32bits (aom_dsp_rtcd.h:855): pure host-memory fill; there is nothing for a
@@ -549,19 +532,11 @@ extern "C" int svt_b200_fullpel_search_batch_host(const uint8_t* src_plane, size
                                                   uint32_t* best_sad, uint32_t* best_mv) {
     require_ready();
     if (n_items <= 0) return n_items == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
-    LaneGuard l;
-    size_t o_src = l->alloc(src_bytes + 8), o_ref = l->alloc(ref_bytes + 8), o_it = l->alloc(sizeof(SvtB200FullpelItem) * n_items);
-    size_t in_end = l->used;
-    size_t o_sad = l->alloc((size_t)n_items * 85 * 4), o_mv = l->alloc((size_t)n_items * 85 * 4);
-    memcpy(l->h<uint8_t>(o_src), src_plane, src_bytes);
-    memcpy(l->h<uint8_t>(o_ref), ref_plane, ref_bytes);
-    memcpy(l->h<uint8_t>(o_it), items, sizeof(SvtB200FullpelItem) * n_items);
-    l->h2d(0, in_end);
-    svt_b200_fullpel_search_batch_dev(l->d<uint8_t>(o_src), l->d<uint8_t>(o_ref), l->d<SvtB200FullpelItem>(o_it), n_items,
-                                      l->d<uint32_t>(o_sad), l->d<uint32_t>(o_mv), l->stream);
-    l->d2h(o_sad, (o_mv + (size_t)n_items * 85 * 4) - o_sad);
-    l->sync();
-    memcpy(best_sad, l->h<uint32_t>(o_sad), (size_t)n_items * 85 * 4);
-    memcpy(best_mv, l->h<uint32_t>(o_mv), (size_t)n_items * 85 * 4);
+    RoundTrip rt;
+    auto src = rt.in(src_plane, src_bytes, src_bytes + 8), ref = rt.in(ref_plane, ref_bytes, ref_bytes + 8);
+    auto it = rt.in(items, n_items);
+    auto sad = rt.out(best_sad, (size_t)n_items * 85), mv = rt.out(best_mv, (size_t)n_items * 85);
+    svt_b200_fullpel_search_batch_dev(rt.dev(src), rt.dev(ref), rt.dev(it), n_items, rt.dev(sad), rt.dev(mv), rt.stream());
+    rt.finish();
     return SVT_B200_OK;
 }

@@ -76,41 +76,29 @@ static void quant_t1(int mode, const int32_t* coeff_ptr, intptr_t n_coeffs, cons
                      const uint8_t* iqm_ptr, int log_scale) {
     require_ready();
     const size_t n = (size_t)n_coeffs;
-    LaneGuard    l;
-    size_t o_c = l->alloc(n * 4), o_scan = l->alloc(n * 2), o_qm = l->alloc(2 * n + 16), o_it = l->alloc(sizeof(SvtB200QuantItem));
-    size_t in_end = l->used;
-    size_t o_q = l->alloc(n * 4), o_dq = l->alloc(n * 4), o_eob = l->alloc(16);
-    memcpy(l->h<int32_t>(o_c), coeff_ptr, n * 4);
-    memcpy(l->h<int16_t>(o_scan), scan, n * 2);
-    SvtB200QuantItem* it = l->h<SvtB200QuantItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->n_coeffs = (uint32_t)n;
-    it->mode = (uint8_t)mode;
-    it->log_scale = (uint8_t)log_scale;
-    it->qm_off = it->iqm_off = SVT_B200_NO_QM;
-    if (qm_ptr) {
-        memcpy(l->h<uint8_t>(o_qm), qm_ptr, n);
-        it->qm_off = 0;
-    }
-    if (iqm_ptr) {
-        memcpy(l->h<uint8_t>(o_qm) + n, iqm_ptr, n);
-        it->iqm_off = (uint32_t)n;
-    }
+    RoundTrip rt;
+    SvtB200QuantItem item{};
+    item.n_coeffs = (uint32_t)n;
+    item.mode = (uint8_t)mode;
+    item.log_scale = (uint8_t)log_scale;
+    item.qm_off = qm_ptr ? 0 : SVT_B200_NO_QM;
+    item.iqm_off = iqm_ptr ? (uint32_t)n : SVT_B200_NO_QM;
     for (int k = 0; k < 2; k++) {
-        it->zbin[k] = zbin_ptr ? zbin_ptr[k] : 0;
-        it->round[k] = round_ptr[k];
-        it->quant[k] = quant_ptr[k];
-        it->quant_shift[k] = quant_shift_ptr ? quant_shift_ptr[k] : 0;
-        it->dequant[k] = dequant_ptr[k];
+        item.zbin[k] = zbin_ptr ? zbin_ptr[k] : 0;
+        item.round[k] = round_ptr[k];
+        item.quant[k] = quant_ptr[k];
+        item.quant_shift[k] = quant_shift_ptr ? quant_shift_ptr[k] : 0;
+        item.dequant[k] = dequant_ptr[k];
     }
-    l->h2d(0, in_end);
-    launch_quant(l->d<int32_t>(o_c), l->d<int32_t>(o_q), l->d<int32_t>(o_dq), l->d<int16_t>(o_scan), nullptr, l->d<uint8_t>(o_qm),
-                 l->d<SvtB200QuantItem>(o_it), 1, l->d<uint16_t>(o_eob), l->stream);
-    l->d2h(o_q, (o_eob + 16) - o_q);
-    l->sync();
-    memcpy(qcoeff_ptr, l->h<int32_t>(o_q), n * 4);
-    memcpy(dqcoeff_ptr, l->h<int32_t>(o_dq), n * 4);
-    *eob_ptr = *l->h<uint16_t>(o_eob);
+    const uint8_t* qm[2] = {qm_ptr, iqm_ptr};
+    auto c = rt.in(coeff_ptr, n);
+    auto sc = rt.in(scan, n);
+    auto m = rt.in_row_list(qm, n, 2, 2 * n + 16);
+    auto it = rt.in(&item, 1);
+    auto q = rt.out(qcoeff_ptr, n), dq = rt.out(dqcoeff_ptr, n);
+    auto eob = rt.out(eob_ptr, 1, 8);
+    launch_quant(rt.dev(c), rt.dev(q), rt.dev(dq), rt.dev(sc), nullptr, rt.dev(m), rt.dev(it), 1, rt.dev(eob), rt.stream());
+    rt.finish();
 }
 
 }  // namespace b200

@@ -329,14 +329,10 @@ extern "C" int svt_b200_sad_search_batch_host(const uint8_t* src_plane, size_t s
                                               SvtB200SadSearchResult* results) {
     require_ready();
     if (n_items <= 0) return n_items == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
-    LaneGuard l;
-    size_t o_src = l->alloc(src_bytes + 8), o_ref = l->alloc(ref_bytes + 8);
-    size_t o_it  = l->alloc(sizeof(SvtB200SadSearchItem) * n_items);
-    size_t in_end = l->used;
-    size_t o_res = l->alloc(sizeof(SvtB200SadSearchResult) * n_items);
-    memcpy(l->h<uint8_t>(o_src), src_plane, src_bytes);
-    memcpy(l->h<uint8_t>(o_ref), ref_plane, ref_bytes);
-    memcpy(l->h<uint8_t>(o_it), items, sizeof(SvtB200SadSearchItem) * n_items);
+    RoundTrip rt;
+    auto src = rt.in(src_plane, src_bytes, src_bytes + 8), ref = rt.in(ref_plane, ref_bytes, ref_bytes + 8);
+    auto it = rt.in(items, n_items);
+    auto res = rt.out(results, n_items);
     size_t smem = 0;
     int max_pos = 0;
     for (int i = 0; i < n_items; i++) {
@@ -346,12 +342,8 @@ extern "C" int svt_b200_sad_search_batch_host(const uint8_t* src_plane, size_t s
         if (s > smem) smem = s;
         if ((int)it.sa_w * it.sa_h > max_pos) max_pos = (int)it.sa_w * it.sa_h;
     }
-    l->h2d(0, in_end);
-    launch_sad_search(l->d<uint8_t>(o_src), l->d<uint8_t>(o_ref), l->d<SvtB200SadSearchItem>(o_it), n_items,
-                      l->d<SvtB200SadSearchResult>(o_res), smem, max_pos, l->stream);
-    l->d2h(o_res, sizeof(SvtB200SadSearchResult) * n_items);
-    l->sync();
-    memcpy(results, l->h<uint8_t>(o_res), sizeof(SvtB200SadSearchResult) * n_items);
+    launch_sad_search(rt.dev(src), rt.dev(ref), rt.dev(it), n_items, rt.dev(res), smem, max_pos, rt.stream());
+    rt.finish();
     return SVT_B200_OK;
 }
 
@@ -363,37 +355,28 @@ extern "C" void svt_b200_sad_loop_kernel(uint8_t* src, uint32_t src_stride, uint
     require_ready();
     *best_sad = 0xffffff;
     if (search_area_width <= 0 || search_area_height <= 0 || block_width == 0 || block_height == 0) return;
-    LaneGuard l;
-    // pack the caller's strided regions densely: block rows at pitch bw, window at its own pitch
+    RoundTrip rt;
+    // the caller's regions as they lie: block rows at src_stride, window at its own pitch
     const size_t src_bytes = (size_t)(block_height - 1) * src_stride + block_width;
     const size_t ref_bytes = (size_t)(search_area_height - 1) * src_stride_raw + (size_t)(block_height - 1) * ref_stride +
                              (size_t)search_area_width + block_width - 1;
-    size_t o_src = l->alloc(src_bytes + 8), o_ref = l->alloc(ref_bytes + 8);
-    size_t o_it  = l->alloc(sizeof(SvtB200SadSearchItem));
-    size_t in_end = l->used;
-    size_t o_res = l->alloc(sizeof(SvtB200SadSearchResult));
-    memcpy(l->h<uint8_t>(o_src), src, src_bytes);
-    memcpy(l->h<uint8_t>(o_ref), ref, ref_bytes);
-    SvtB200SadSearchItem* it = l->h<SvtB200SadSearchItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->src_off = 0;
-    it->ref_off = 0;
-    it->src_stride = src_stride;
-    it->ref_stride = ref_stride;
-    it->ref_step = src_stride_raw;
-    it->block_w = (uint16_t)block_width;
-    it->block_h = (uint16_t)block_height;
-    it->sa_w = search_area_width;
-    it->sa_h = search_area_height;
-    it->skip_search_line = skip_search_line;
+    SvtB200SadSearchItem item{};
+    item.src_stride = src_stride;
+    item.ref_stride = ref_stride;
+    item.ref_step = src_stride_raw;
+    item.block_w = (uint16_t)block_width;
+    item.block_h = (uint16_t)block_height;
+    item.sa_w = search_area_width;
+    item.sa_h = search_area_height;
+    item.skip_search_line = skip_search_line;
+    auto s = rt.in(src, src_bytes, src_bytes + 8), win = rt.in(ref, ref_bytes, ref_bytes + 8);
+    auto it = rt.in(&item, 1);
+    auto res = rt.out<SvtB200SadSearchResult>(nullptr, 1);
     int k = (src_stride_raw && ref_stride % src_stride_raw == 0) ? (int)(ref_stride / src_stride_raw) : 1;
     size_t smem = smem_needed((int)block_width, (int)block_height, search_area_width, search_area_height, k);
-    l->h2d(0, in_end);
-    launch_sad_search(l->d<uint8_t>(o_src), l->d<uint8_t>(o_ref), l->d<SvtB200SadSearchItem>(o_it), 1,
-                      l->d<SvtB200SadSearchResult>(o_res), smem, (int)search_area_width * search_area_height, l->stream);
-    l->d2h(o_res, sizeof(SvtB200SadSearchResult));
-    l->sync();
-    const SvtB200SadSearchResult* r = l->h<SvtB200SadSearchResult>(o_res);
+    launch_sad_search(rt.dev(s), rt.dev(win), rt.dev(it), 1, rt.dev(res), smem, (int)search_area_width * search_area_height, rt.stream());
+    rt.finish();
+    const SvtB200SadSearchResult* r = rt.host(res);
     if (r->x >= 0) {
         *best_sad        = r->best_sad;
         *x_search_center = r->x;
@@ -405,20 +388,14 @@ extern "C" uint32_t svt_b200_nxm_sad_kernel(const uint8_t* src, uint32_t src_str
                                             uint32_t ref_stride, uint32_t height, uint32_t width) {
     require_ready();
     if (!height || !width) return 0;
-    LaneGuard l;
+    RoundTrip rt;
     const size_t sb = (size_t)(height - 1) * src_stride + width, rb = (size_t)(height - 1) * ref_stride + width;
-    size_t o_src = l->alloc(sb), o_ref = l->alloc(rb);
-    size_t in_end = l->used;
-    size_t o_out = l->alloc(4);
-    memcpy(l->h<uint8_t>(o_src), src, sb);
-    memcpy(l->h<uint8_t>(o_ref), ref, rb);
-    l->h2d(0, in_end);
-    nxm_sad_kernel<<<1, 256, 0, l->stream>>>(l->d<uint8_t>(o_src), src_stride, l->d<uint8_t>(o_ref), ref_stride, height,
-                                             width, l->d<uint32_t>(o_out));
+    auto s = rt.in(src, sb), r = rt.in(ref, rb);
+    auto out = rt.out<uint32_t>(nullptr, 1);
+    nxm_sad_kernel<<<1, 256, 0, rt.stream()>>>(rt.dev(s), src_stride, rt.dev(r), ref_stride, height, width, rt.dev(out));
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, 4);
-    l->sync();
-    return *l->h<uint32_t>(o_out);
+    rt.finish();
+    return *rt.host(out);
 }
 
 // ---- T1: svt_aom_sadMxN / svt_aom_sadMxNx4d (aom_dsp_rtcd.h:275-403; C: compute_sad_c.c:104-215) ----

@@ -168,41 +168,29 @@ static void launch_sgr(const PIX* d_dgd, const SvtB200SgrUnit* d_units, int n, i
     B200_LAUNCH_CHECK();
 }
 
-// stage (w+6)x(h+6) pixels around dat into the lane; returns offset of pixel (0,0)
-template <typename PIX>
-static size_t stage_ext(Lane* l, const PIX* dgd, int w, int h, int stride, int border, size_t* pitch) {
-    const int tw = w + 2 * border, th = h + 2 * border;
-    size_t o = l->alloc((size_t)tw * th * sizeof(PIX));
-    for (int r = 0; r < th; r++) memcpy(l->h<PIX>(o) + (size_t)r * tw, dgd + (ptrdiff_t)(r - border) * stride - border, tw * sizeof(PIX));
-    *pitch = tw;
-    return o;
+// the unit of a w x h block staged with its 3-pixel border at pitch w + 6, filter outputs at pitch w
+static SvtB200SgrUnit t1_unit(int w, int h, int idx) {
+    SvtB200SgrUnit u{};
+    u.dgd_off = 3 * (w + 6) + 3;
+    u.dgd_stride = w + 6;
+    u.flt_stride = w;
+    u.w = (uint16_t)w;
+    u.h = (uint16_t)h;
+    u.params_idx = (uint16_t)idx;
+    return u;
 }
 
 template <typename PIX>
 static void sgr_t1(const PIX* dgd, int w, int h, int stride, int32_t* flt0, int32_t* flt1, int flt_stride, int idx, int bd) {
     require_ready();
-    LaneGuard l;
-    size_t pitch;
-    size_t o_d = stage_ext<PIX>(l.l, dgd, w, h, stride, 3, &pitch), o_u = l->alloc(sizeof(SvtB200SgrUnit));
-    size_t in_end = l->used;
-    size_t o_f0 = l->alloc((size_t)w * h * 4), o_f1 = l->alloc((size_t)w * h * 4);
-    SvtB200SgrUnit* u = l->h<SvtB200SgrUnit>(o_u);
-    memset(u, 0, sizeof(*u));
-    u->dgd_off = 3 * pitch + 3;
-    u->dgd_stride = (int32_t)pitch;
-    u->flt_stride = w;
-    u->w = (uint16_t)w;
-    u->h = (uint16_t)h;
-    u->params_idx = (uint16_t)idx;
-    l->h2d(0, in_end);
-    launch_sgr<PIX>(l->d<PIX>(o_d), l->d<SvtB200SgrUnit>(o_u), 1, l->d<int32_t>(o_f0), l->d<int32_t>(o_f1), bd, w, h, l->stream);
-    l->d2h(o_f0, (o_f1 + (size_t)w * h * 4) - o_f0);
-    l->sync();
-    const int* prm = h_sgr_params + 4 * idx;
-    for (int r = 0; r < h; r++) {
-        if (prm[0] > 0) memcpy(flt0 + (size_t)r * flt_stride, l->h<int32_t>(o_f0) + (size_t)r * w, w * 4);
-        if (prm[1] > 0) memcpy(flt1 + (size_t)r * flt_stride, l->h<int32_t>(o_f1) + (size_t)r * w, w * 4);
-    }
+    RoundTrip rt;
+    const SvtB200SgrUnit unit = t1_unit(w, h, idx);
+    const int* prm = h_sgr_params + 4 * idx;  // a filter whose radius is 0 leaves its output alone
+    auto d = rt.in_rows(dgd - 3 * stride - 3, stride, w + 6, h + 6);
+    auto u = rt.in(&unit, 1);
+    auto f0 = rt.out_rows(prm[0] > 0 ? flt0 : nullptr, flt_stride, w, h), f1 = rt.out_rows(prm[1] > 0 ? flt1 : nullptr, flt_stride, w, h);
+    launch_sgr<PIX>(rt.dev(d), rt.dev(u), 1, rt.dev(f0), rt.dev(f1), bd, w, h, rt.stream());
+    rt.finish();
 }
 
 template <typename PIX>
@@ -213,83 +201,52 @@ static void sgr_apply_t1(const PIX* dat, int w, int h, int stride, int eps, cons
     if (prm[0] == 0) { xq[0] = 0; xq[1] = 128 - xqd[1]; }
     else if (prm[1] == 0) { xq[0] = xqd[0]; xq[1] = 0; }
     else { xq[0] = xqd[0]; xq[1] = 128 - xq[0] - xqd[1]; }
-    LaneGuard l;
-    size_t pitch;
-    size_t o_d = stage_ext<PIX>(l.l, dat, w, h, stride, 3, &pitch), o_u = l->alloc(sizeof(SvtB200SgrUnit));
-    size_t in_end = l->used;
-    size_t o_f0 = l->alloc((size_t)w * h * 4), o_f1 = l->alloc((size_t)w * h * 4), o_o = l->alloc((size_t)w * h * sizeof(PIX));
-    SvtB200SgrUnit* u = l->h<SvtB200SgrUnit>(o_u);
-    memset(u, 0, sizeof(*u));
-    u->dgd_off = 3 * pitch + 3;
-    u->dgd_stride = (int32_t)pitch;
-    u->flt_stride = w;
-    u->w = (uint16_t)w;
-    u->h = (uint16_t)h;
-    u->params_idx = (uint16_t)eps;
-    l->h2d(0, in_end);
-    launch_sgr<PIX>(l->d<PIX>(o_d), l->d<SvtB200SgrUnit>(o_u), 1, l->d<int32_t>(o_f0), l->d<int32_t>(o_f1), bd, w, h, l->stream);
-    sgr_project_kernel<PIX><<<grid_for((w * h + 255) / 256, 8), 256, 0, l->stream>>>(l->d<PIX>(o_d) + 3 * pitch + 3, w, h, (int)pitch, l->d<int32_t>(o_f0),
-                                                                                  l->d<int32_t>(o_f1), xq[0], xq[1], prm[0], prm[1], l->d<PIX>(o_o), w, bd);
+    RoundTrip rt;
+    const SvtB200SgrUnit unit = t1_unit(w, h, eps);
+    auto d = rt.in_rows(dat - 3 * stride - 3, stride, w + 6, h + 6);
+    auto u = rt.in(&unit, 1);
+    auto o = rt.out_rows(dst, dst_stride, w, h);
+    auto f0 = rt.scratch<int32_t>((size_t)w * h), f1 = rt.scratch<int32_t>((size_t)w * h);
+    launch_sgr<PIX>(rt.dev(d), rt.dev(u), 1, rt.dev(f0), rt.dev(f1), bd, w, h, rt.stream());
+    sgr_project_kernel<PIX><<<grid_for((w * h + 255) / 256, 8), 256, 0, rt.stream()>>>(rt.dev(d) + 3 * (w + 6) + 3, w, h, w + 6, rt.dev(f0),
+                                                                                    rt.dev(f1), xq[0], xq[1], prm[0], prm[1], rt.dev(o), w, bd);
     B200_LAUNCH_CHECK();
-    l->d2h(o_o, (size_t)w * h * sizeof(PIX));
-    l->sync();
-    for (int r = 0; r < h; r++) memcpy(dst + (size_t)r * dst_stride, l->h<PIX>(o_o) + (size_t)r * w, w * sizeof(PIX));
+    rt.finish();
 }
 
-struct ProjStage { size_t o_src, o_dat, o_f0, o_f1; };
-template <typename PIX>
-static ProjStage stage_proj(Lane* l, const PIX* src, int w, int h, int ss, const PIX* dat, int ds, const int32_t* flt0, int f0s,
-                            const int32_t* flt1, int f1s, int r0, int r1) {
-    ProjStage p;
-    p.o_src = l->alloc((size_t)w * h * sizeof(PIX));
-    p.o_dat = l->alloc((size_t)w * h * sizeof(PIX));
-    p.o_f0 = l->alloc((size_t)w * h * 4);
-    p.o_f1 = l->alloc((size_t)w * h * 4);
-    for (int r = 0; r < h; r++) {
-        memcpy(l->h<PIX>(p.o_src) + (size_t)r * w, src + (size_t)r * ss, w * sizeof(PIX));
-        memcpy(l->h<PIX>(p.o_dat) + (size_t)r * w, dat + (size_t)r * ds, w * sizeof(PIX));
-        if (r0 > 0) memcpy(l->h<int32_t>(p.o_f0) + (size_t)r * w, flt0 + (size_t)r * f0s, w * 4);
-        if (r1 > 0) memcpy(l->h<int32_t>(p.o_f1) + (size_t)r * w, flt1 + (size_t)r * f1s, w * 4);
-    }
-    return p;
-}
-
+// the projection calls read src, dat and the outputs of the filters whose radius is positive, each at pitch w
 template <typename PIX, bool HBD_FORM>
 static int64_t proj_error_t1(const PIX* src, int w, int h, int ss, const PIX* dat, int ds, int32_t* flt0, int f0s, int32_t* flt1, int f1s,
                              int32_t xq[2], const int32_t* params) {
     require_ready();
-    LaneGuard l;
-    ProjStage p = stage_proj<PIX>(l.l, src, w, h, ss, dat, ds, flt0, f0s, flt1, f1s, params[0], params[1]);
-    size_t o_out = l->alloc(8);
-    *l->h<int64_t>(o_out) = 0;
-    l->h2d(0, l->used);
-    proj_error_kernel<PIX, HBD_FORM><<<grid_for((w * h + 255) / 256, 8), 256, 0, l->stream>>>(
-        l->d<PIX>(p.o_src), w, h, w, l->d<PIX>(p.o_dat), w, l->d<int32_t>(p.o_f0), w, l->d<int32_t>(p.o_f1), w, xq[0], xq[1], params[0], params[1],
-        l->d<long long>(o_out));
+    RoundTrip rt;
+    auto s = rt.in_rows(src, ss, w, h), d = rt.in_rows(dat, ds, w, h);
+    auto f0 = rt.in_rows(params[0] > 0 ? flt0 : nullptr, f0s, w, h), f1 = rt.in_rows(params[1] > 0 ? flt1 : nullptr, f1s, w, h);
+    int64_t err = 0;
+    auto e = rt.inout(&err, 1);
+    proj_error_kernel<PIX, HBD_FORM><<<grid_for((w * h + 255) / 256, 8), 256, 0, rt.stream()>>>(
+        rt.dev(s), w, h, w, rt.dev(d), w, rt.dev(f0), w, rt.dev(f1), w, xq[0], xq[1], params[0], params[1], (long long*)rt.dev(e));
     B200_LAUNCH_CHECK();
-    l->d2h(o_out, 8);
-    l->sync();
-    return *l->h<int64_t>(o_out);
+    rt.finish();
+    return err;
 }
 
 template <typename PIX>
 static void proj_subspace_t1(const PIX* src, int w, int h, int ss, const PIX* dat, int ds, int32_t* flt0, int f0s, int32_t* flt1, int f1s,
                              int* xq, const int32_t* params) {
     require_ready();
-    LaneGuard l;
-    ProjStage p = stage_proj<PIX>(l.l, src, w, h, ss, dat, ds, flt0, f0s, flt1, f1s, params[0], params[1]);
-    size_t o_s = l->alloc(48);
-    memset(l->h<uint8_t>(o_s), 0, 48);
-    l->h2d(0, l->used);
-    proj_subspace_sums_kernel<PIX><<<grid_for((w * h + 255) / 256, 8), 256, 0, l->stream>>>(l->d<PIX>(p.o_src), w, h, w, l->d<PIX>(p.o_dat), w,
-                                                                                          l->d<int32_t>(p.o_f0), w, l->d<int32_t>(p.o_f1), w,
-                                                                                          params[0], params[1], l->d<long long>(o_s));
+    RoundTrip rt;
+    auto s = rt.in_rows(src, ss, w, h), d = rt.in_rows(dat, ds, w, h);
+    auto f0 = rt.in_rows(params[0] > 0 ? flt0 : nullptr, f0s, w, h), f1 = rt.in_rows(params[1] > 0 ? flt1 : nullptr, f1s, w, h);
+    long long sums[6] = {};  // five moments, then the solver's two ints
+    auto sm = rt.inout(sums, 6);
+    proj_subspace_sums_kernel<PIX><<<grid_for((w * h + 255) / 256, 8), 256, 0, rt.stream()>>>(rt.dev(s), w, h, w, rt.dev(d), w, rt.dev(f0), w,
+                                                                                            rt.dev(f1), w, params[0], params[1], rt.dev(sm));
     B200_LAUNCH_CHECK();
-    proj_subspace_solve_kernel<<<1, 1, 0, l->stream>>>(l->d<long long>(o_s), w * h, params[0], params[1], (int*)(l->d<long long>(o_s) + 5));
+    proj_subspace_solve_kernel<<<1, 1, 0, rt.stream()>>>(rt.dev(sm), w * h, params[0], params[1], (int*)(rt.dev(sm) + 5));
     B200_LAUNCH_CHECK();
-    l->d2h(o_s, 48);
-    l->sync();
-    const int* r = (const int*)(l->h<long long>(o_s) + 5);
+    rt.finish();
+    const int* r = (const int*)(sums + 5);
     xq[0] = r[0];
     xq[1] = r[1];
 }

@@ -768,25 +768,20 @@ extern "C" void svt_b200_fwd_txfm2d_partial(int16_t* input, int32_t* output, uin
         fprintf(stderr, "[svt_b200] FATAL: invalid (tx_size=%d, tx_type=%d)\n", tx_size, tx_type);
         abort();
     }
-    LaneGuard l;
-    size_t o_src = l->alloc((size_t)W * H * 2), o_it = l->alloc(sizeof(SvtB200FwdTxfmItem));
-    size_t in_end = l->used;
-    size_t o_dst = l->alloc((size_t)W * H * 4);
-    for (int r = 0; r < H; r++) memcpy(l->h<int16_t>(o_src) + r * W, input + (size_t)r * input_stride, W * 2);
-    SvtB200FwdTxfmItem* it = l->h<SvtB200FwdTxfmItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->src_stride = W;
-    it->tx_size = (uint8_t)tx_size;
-    it->tx_type = (uint8_t)tx_type;
-    it->reserved = (uint16_t)(level << 1);
-    l->h2d(0, in_end);
+    RoundTrip rt;
+    SvtB200FwdTxfmItem item{};
+    item.src_stride = W;
+    item.tx_size = (uint8_t)tx_size;
+    item.tx_type = (uint8_t)tx_type;
+    item.reserved = (uint16_t)(level << 1);
+    auto src = rt.in_rows(input, input_stride, W, H);
+    auto it = rt.in(&item, 1);
+    auto dst = rt.out(output, (size_t)W * H);
     TxfmBufs b;
-    b.residual = l->d<int16_t>(o_src);
-    b.coef     = l->d<int32_t>(o_dst);
-    launch_class<Forward, uint8_t>(tx_class(tx_size), b, l->d<SvtB200FwdTxfmItem>(o_it), 1, nullptr, l->stream);
-    l->d2h(o_dst, (size_t)W * H * 4);
-    l->sync();
-    memcpy(output, l->h<int32_t>(o_dst), (size_t)W * H * 4);
+    b.residual = rt.dev(src);
+    b.coef     = rt.dev(dst);
+    launch_class<Forward, uint8_t>(tx_class(tx_size), b, rt.dev(it), 1, nullptr, rt.stream());
+    rt.finish();
 }
 
 // ---- T1: svt_av1_inv_txfm2d_add_WxH (common_dsp_rtcd.h:106-142; C: inv_transforms.c:2545-2716) on 16-bit pixels, and
@@ -801,27 +796,22 @@ static void inv_txfm_add_t1(const int32_t* input, const PIX* pred, int32_t strid
         fprintf(stderr, "[svt_b200] FATAL: invalid (tx_size=%d, tx_type=%d)\n", tx_size, tx_type);
         abort();
     }
-    LaneGuard l;
-    size_t o_in = l->alloc((size_t)Wp * Hp * 4), o_pred = l->alloc((size_t)W * H * sizeof(PIX)), o_it = l->alloc(sizeof(SvtB200InvTxfmItem));
-    size_t in_end = l->used;
-    size_t o_out = l->alloc((size_t)W * H * sizeof(PIX));
-    memcpy(l->h<int32_t>(o_in), input, (size_t)Wp * Hp * 4);
-    for (int r = 0; r < H; r++) memcpy(l->h<PIX>(o_pred) + r * W, pred + (size_t)r * stride_r, W * sizeof(PIX));
-    SvtB200InvTxfmItem* it = l->h<SvtB200InvTxfmItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->pred_stride = it->recon_stride = W;
-    it->tx_size = (uint8_t)tx_size;
-    it->tx_type = (uint8_t)tx_type;
-    it->bd = (uint8_t)bd;
-    l->h2d(0, in_end);
+    RoundTrip rt;
+    SvtB200InvTxfmItem item{};
+    item.pred_stride = item.recon_stride = W;
+    item.tx_size = (uint8_t)tx_size;
+    item.tx_type = (uint8_t)tx_type;
+    item.bd = (uint8_t)bd;
+    auto in = rt.in(input, (size_t)Wp * Hp);
+    auto pr = rt.in_rows(pred, stride_r, W, H);
+    auto it = rt.in(&item, 1);
+    auto rec = rt.out_rows(out, stride_w, W, H);
     TxfmBufs b;
-    b.pred  = l->d<PIX>(o_pred);
-    b.recon = l->d<PIX>(o_out);
-    b.dq_in = l->d<int32_t>(o_in);
-    launch_class<Inverse, PIX>(tx_class(tx_size), b, l->d<SvtB200InvTxfmItem>(o_it), 1, nullptr, l->stream);
-    l->d2h(o_out, (size_t)W * H * sizeof(PIX));
-    l->sync();
-    for (int r = 0; r < H; r++) memcpy(out + (size_t)r * stride_w, l->h<PIX>(o_out) + r * W, W * sizeof(PIX));
+    b.pred  = rt.dev(pr);
+    b.recon = rt.dev(rec);
+    b.dq_in = rt.dev(in);
+    launch_class<Inverse, PIX>(tx_class(tx_size), b, rt.dev(it), 1, nullptr, rt.stream());
+    rt.finish();
 }
 extern "C" void svt_b200_inv_txfm2d_add(const int32_t* input, uint16_t* output_r, int32_t stride_r, uint16_t* output_w,
                                         int32_t stride_w, int tx_type, int tx_size, int32_t bd) {
@@ -837,30 +827,27 @@ extern "C" int svt_b200_fwd_txfm_batch_host(const int16_t* residual, size_t resi
                                             const SvtB200FwdTxfmItem* items, int n_items) {
     require_ready();
     if (n_items <= 0) return n_items == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
-    LaneGuard l;
-    size_t o_src = l->alloc(residual_elems * 2), o_it = l->alloc(sizeof(SvtB200FwdTxfmItem) * n_items);
-    size_t in_end = l->used;
-    size_t o_dst = l->alloc(coeff_elems * 4);
-    memcpy(l->h<int16_t>(o_src), residual, residual_elems * 2);
-    SvtB200FwdTxfmItem* hi = l->h<SvtB200FwdTxfmItem>(o_it);
     int cnt[SVT_B200_TXFM_CLASSES] = {0, 0, 0, 0, 0}, pos[SVT_B200_TXFM_CLASSES];
     for (int i = 0; i < n_items; i++) {
         if (items[i].tx_size >= 19 || !host_txcfg(items[i].tx_size, items[i].tx_type).valid) return SVT_B200_ERR_BAD_ARG;
         cnt[tx_class(items[i].tx_size)]++;
     }
+    RoundTrip rt;
+    auto src = rt.in(residual, residual_elems);
+    auto it = rt.in<SvtB200FwdTxfmItem>(nullptr, n_items);
+    auto dst = rt.out<int32_t>(nullptr, coeff_elems);
+    SvtB200FwdTxfmItem* hi = rt.fill(it);  // the items grouped by transform class
     for (int c = 0, first = 0; c < SVT_B200_TXFM_CLASSES; first += cnt[c], c++) pos[c] = first;
     for (int i = 0; i < n_items; i++) hi[pos[tx_class(items[i].tx_size)]++] = items[i];
-    l->h2d(0, in_end);
     TxfmBufs b;
-    b.residual = l->d<int16_t>(o_src);
-    b.coef     = l->d<int32_t>(o_dst);
-    launch_batch<Forward, uint8_t>(b, l->d<SvtB200FwdTxfmItem>(o_it), cnt, nullptr, l->stream);
-    l->d2h(o_dst, coeff_elems * 4);
-    l->sync();
+    b.residual = rt.dev(src);
+    b.coef     = rt.dev(dst);
+    launch_batch<Forward, uint8_t>(b, rt.dev(it), cnt, nullptr, rt.stream());
+    rt.finish();
     // only the regions the items cover were written; copy those back
     for (int i = 0; i < n_items; i++) {
         const int W = tx_w(items[i].tx_size), H = tx_h(items[i].tx_size);
-        memcpy(coeff + items[i].dst_off, l->h<int32_t>(o_dst) + items[i].dst_off, (size_t)W * H * 4);
+        memcpy(coeff + items[i].dst_off, rt.host(dst) + items[i].dst_off, (size_t)W * H * 4);
     }
     return SVT_B200_OK;
 }
@@ -897,17 +884,13 @@ handle_transform_kernel(int32_t* __restrict__ buf, int W, int H, int with_energy
 
 static uint64_t handle_transform_t1(int32_t* output, int W, int H, int with_energy) {
     require_ready();
-    LaneGuard l;
-    const size_t n = (size_t)W * H;
-    size_t o_buf = l->alloc(n * 4), o_e = l->alloc(16);
-    memcpy(l->h<int32_t>(o_buf), output, n * 4);
-    l->h2d(o_buf, n * 4);
-    handle_transform_kernel<<<1, 256, 0, l->stream>>>(l->d<int32_t>(o_buf), W, H, with_energy, l->d<unsigned long long>(o_e));
+    RoundTrip rt;
+    auto buf = rt.inout(output, (size_t)W * H);
+    auto e = rt.out<unsigned long long>(nullptr, 2);
+    handle_transform_kernel<<<1, 256, 0, rt.stream()>>>(rt.dev(buf), W, H, with_energy, rt.dev(e));
     B200_LAUNCH_CHECK();
-    l->d2h(o_buf, (o_e + 16) - o_buf);
-    l->sync();
-    memcpy(output, l->h<int32_t>(o_buf), n * 4);
-    return (uint64_t)*l->h<unsigned long long>(o_e);
+    rt.finish();
+    return (uint64_t)*rt.host(e);
 }
 #define B200_HANDLE(WxH, W, H)                                                                                    \
     extern "C" uint64_t svt_b200_handle_transform##WxH(int32_t* output) { return handle_transform_t1(output, W, H, 1); } \

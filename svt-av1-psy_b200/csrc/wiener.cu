@@ -428,59 +428,45 @@ static void stats_t1(int wiener_win, const PIX* dgd, const PIX* src, int h_start
     const int half = wiener_win >> 1, win2 = wiener_win * wiener_win;
     const int w = h_end - h_start, h = v_end - v_start;
     const int dw = w + 2 * half, dh = h + 2 * half;
-    LaneGuard l;
-    size_t o_d = l->alloc((size_t)dw * dh * sizeof(PIX)), o_s = l->alloc((size_t)w * h * sizeof(PIX)), o_it = l->alloc(sizeof(SvtB200StatsItem));
-    size_t in_end = l->used;
-    size_t o_M = l->alloc(49 * 8), o_H = l->alloc(2401 * 8), o_acc = l->alloc((size_t)kLagItemWords * 8), o_avg = l->alloc(16);
-    for (int r = 0; r < dh; r++)
-        memcpy(l->h<PIX>(o_d) + (size_t)r * dw, dgd + (ptrdiff_t)(v_start - half + r) * dgd_stride + h_start - half, dw * sizeof(PIX));
-    for (int r = 0; r < h; r++) memcpy(l->h<PIX>(o_s) + (size_t)r * w, src + (ptrdiff_t)(v_start + r) * src_stride + h_start, w * sizeof(PIX));
-    SvtB200StatsItem* it = l->h<SvtB200StatsItem>(o_it);
-    memset(it, 0, sizeof(*it));
-    it->dgd_off = (uint64_t)half * dw + half;  // (v_start, h_start) of the packed copy
-    it->src_off = 0;
-    it->dgd_stride = dw;
-    it->src_stride = w;
-    it->h_start = 0;
-    it->h_end = w;
-    it->v_start = 0;
-    it->v_end = h;
-    it->wiener_win = wiener_win;
-    l->h2d(0, in_end);
-    launch_stats<PIX>(l->d<PIX>(o_d), l->d<PIX>(o_s), l->d<SvtB200StatsItem>(o_it), 1, bd, l->d<long long>(o_M), l->d<long long>(o_H),
-                      l->d<long long>(o_acc), l->d<unsigned long long>(o_avg), l->stream);
-    l->d2h(o_M, (o_H + 2401 * 8) - o_M);
-    l->sync();
-    memcpy(M, l->h<int64_t>(o_M), (size_t)win2 * 8);
-    memcpy(H, l->h<int64_t>(o_H), (size_t)win2 * win2 * 8);
+    RoundTrip rt;
+    SvtB200StatsItem item{};
+    item.dgd_off = (uint64_t)half * dw + half;  // (v_start, h_start) of the packed copy
+    item.dgd_stride = dw;
+    item.src_stride = w;
+    item.h_end = w;
+    item.v_end = h;
+    item.wiener_win = wiener_win;
+    auto d = rt.in_rows(dgd + (ptrdiff_t)(v_start - half) * dgd_stride + h_start - half, dgd_stride, dw, dh);
+    auto s = rt.in_rows(src + (ptrdiff_t)v_start * src_stride + h_start, src_stride, w, h);
+    auto it = rt.in(&item, 1);
+    auto m = rt.out(M, win2, 49), hh = rt.out(H, (size_t)win2 * win2, 2401);
+    auto acc = rt.scratch<long long>(kLagItemWords);
+    auto avg = rt.scratch<unsigned long long>(2);
+    launch_stats<PIX>(rt.dev(d), rt.dev(s), rt.dev(it), 1, bd, (long long*)rt.dev(m), (long long*)rt.dev(hh), rt.dev(acc), rt.dev(avg),
+                      rt.stream());
+    rt.finish();
 }
 
 template <typename PIX>
 static void wiener_t1(const PIX* src, ptrdiff_t src_stride, PIX* dst, ptrdiff_t dst_stride, const int16_t* fx, const int16_t* fy, int w,
                       int h, int round0, int round1, int bd, int lbd_rows) {
     require_ready();
-    LaneGuard l;
+    RoundTrip rt;
     const int sw = w + 8, sh = h + 7;
-    size_t o_s = l->alloc((size_t)sw * sh * sizeof(PIX)), o_u = l->alloc(sizeof(SvtB200WienerUnit));
-    size_t in_end = l->used;
-    size_t o_d = l->alloc((size_t)w * h * sizeof(PIX));
-    for (int r = 0; r < sh; r++) memcpy(l->h<PIX>(o_s) + (size_t)r * sw, src + (ptrdiff_t)(r - 3) * src_stride - 3, sw * sizeof(PIX));
-    SvtB200WienerUnit* u = l->h<SvtB200WienerUnit>(o_u);
-    memset(u, 0, sizeof(*u));
-    u->src_off = (uint64_t)3 * sw + 3;
-    u->dst_off = 0;
-    u->src_stride = sw;
-    u->dst_stride = w;
-    u->w = (uint16_t)w;
-    u->h = (uint16_t)h;
-    memcpy(u->hfilter, fx, 16);
-    memcpy(u->vfilter, fy, 16);
-    l->h2d(0, in_end);
-    wiener_convolve_kernel<PIX><<<1, 256, 0, l->stream>>>(l->d<PIX>(o_s), l->d<PIX>(o_d), l->d<SvtB200WienerUnit>(o_u), 1, bd, round0, round1, lbd_rows);
+    SvtB200WienerUnit unit{};
+    unit.src_off = (uint64_t)3 * sw + 3;
+    unit.src_stride = sw;
+    unit.dst_stride = w;
+    unit.w = (uint16_t)w;
+    unit.h = (uint16_t)h;
+    memcpy(unit.hfilter, fx, 16);
+    memcpy(unit.vfilter, fy, 16);
+    auto s = rt.in_rows(src - 3 * src_stride - 3, src_stride, sw, sh);
+    auto u = rt.in(&unit, 1);
+    auto d = rt.out_rows(dst, dst_stride, w, h);
+    wiener_convolve_kernel<PIX><<<1, 256, 0, rt.stream()>>>(rt.dev(s), rt.dev(d), rt.dev(u), 1, bd, round0, round1, lbd_rows);
     B200_LAUNCH_CHECK();
-    l->d2h(o_d, (size_t)w * h * sizeof(PIX));
-    l->sync();
-    for (int r = 0; r < h; r++) memcpy(dst + (ptrdiff_t)r * dst_stride, l->h<PIX>(o_d) + (size_t)r * w, w * sizeof(PIX));
+    rt.finish();
 }
 
 }  // namespace b200
