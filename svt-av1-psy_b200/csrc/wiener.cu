@@ -32,8 +32,8 @@ template <typename PIX>
 __global__ void __launch_bounds__(256)
 wiener_convolve_kernel(const PIX* __restrict__ src_base, PIX* __restrict__ dst_base, const SvtB200WienerUnit* __restrict__ units,
                        int n_units, int bd, int round0, int round1, int lbd_rows) {
-    __shared__ __align__(16) uint16_t s_src[(64 + 8) * (64 + 8)];
-    __shared__ __align__(16) uint16_t s_tmp[(64 + 8) * 64];
+    __shared__ __align__(16) PIX      s_src[kWienerTileRows * kWienerTilePitch];
+    __shared__ __align__(16) uint16_t s_tmp[kWienerTileRows * 64];
     for (int it = blockIdx.x; it < n_units; it += gridDim.x) {
         const SvtB200WienerUnit u = units[it];
         const int w = u.w, h = u.h;
@@ -45,7 +45,7 @@ wiener_convolve_kernel(const PIX* __restrict__ src_base, PIX* __restrict__ dst_b
             const int r = i / sw, c = i - r * sw;
             // the 8th tap is read by the reference too (multiplied by its coefficient); the column
             // w+4 it touches on the last pixel is part of the caller's extended border
-            s_src[r * 72 + c] = (uint16_t)src[(ptrdiff_t)(r - 3) * u.src_stride + (c - 3)];
+            s_src[r * kWienerTilePitch + c + 1] = src[(ptrdiff_t)(r - 3) * u.src_stride + (c - 3)];
         }
         __syncthreads();
         wiener_unit_compute<PIX>(s_src, s_tmp, dst, u.dst_stride, w, h, u.hfilter, u.vfilter, bd, round0, round1, lbd_rows);
