@@ -8,11 +8,13 @@
 // 106-352: CDEF_VERY_LARGE outside the frame, pre-filter neighbours inside).
 //
 // H100 mapping (T2): a frame-wide kernel finds direction and variance of every non-skip 8x8 (one
-// thread per block, the 64 pixels in registers).  Search and apply run one 128-thread CTA per (64x64
-// filter block, plane): the padded 16-bit tile of the plane, (fbs + 6) x (fbs + 16) for a filter block of
-// fbs x fbs pixels in that plane, is staged in shared memory once, and a thread owns a row segment of one
-// block (luma: a processed 8-pixel row of an 8x8, chroma: a 4-pixel row of a 4x4), so the tap offsets of
-// the block's direction and the per-strength constants are built once per segment, not per pixel.  A
+// thread per block, the 64 pixels in registers).  Search and apply run one 128-thread CTA per 64x64 filter
+// block and luma, and one per filter block and both chroma planes (which share the block list, directions,
+// strengths and damping): the padded 16-bit tile of each plane, (fbs + 6) x (fbs + 16) for a filter block of
+// fbs x fbs pixels in that plane, is staged in shared memory once, in words of 8 pixels, and a thread owns a row
+// segment of one block (luma: a processed 8-pixel row of an 8x8, chroma: a 4-pixel row of a 4x4 in Cb and the
+// same row in Cr), so the tap offsets of the block's direction and the per-strength constants are built once per
+// segment, not per pixel.  The search evaluates two pixels per step (luma: neighbours, chroma: one per plane).  A
 // pixel's 12 taps are fetched once per direction, as signed differences and magnitudes packed two per
 // register, and shared by all candidate strengths; the filter sum is separable into a primary and a
 // secondary half, each evaluated once per distinct strength value with native packed 16-bit min/max/add
@@ -297,31 +299,64 @@ __global__ void search_one_dual_kernel(const unsigned long long* mse0, const uns
 // ------------------------------------------------------------------------------------------------
 constexpr int kT2Threads = 128;  // threads of a search / apply CTA
 constexpr int kGChunk    = 8;    // candidate strengths whose moments a search thread keeps in registers at once
+constexpr int kTPC       = 48;   // chroma tile pitch in uint16 (32 + 2*8, rows 16-B aligned)
+constexpr int kTileC     = (32 + 6) * kTPC;  // one chroma tile; the Cr tile follows the Cb tile
+static_assert(2 * kTileC <= kTileRows * kTP, "both chroma tiles fit where the luma tile goes");
 
+// 8 pixels at p as 8 uint16 (p aligned to 8 pixels)
 template <typename PIX>
-__device__ void stage_cdef_tile(uint16_t* tile, const PIX* plane, int stride, int fbr, int fbc, int nvfb, int nhfb, int fbs,
-                                int vsz, int hsz) {
-    // tile origin (row 3, col 8) = first pixel of the filter block; everything outside the copied
-    // rectangle is CDEF_VERY_LARGE (cdef_process.c:211-230).  Only the (fbs + 6) x (fbs + 16) pixels the
-    // filter can read are written.  One pass, two pixels per thread and store.
+__device__ __forceinline__ uint4 cdef_load_word8(const PIX* p) {
+    if (sizeof(PIX) == 1) {
+        const uint2 w = *reinterpret_cast<const uint2*>(p);
+        return make_uint4(__byte_perm(w.x, 0, 0x4140), __byte_perm(w.x, 0, 0x4342), __byte_perm(w.y, 0, 0x4140), __byte_perm(w.y, 0, 0x4342));
+    }
+    return *reinterpret_cast<const uint4*>(p);
+}
+
+// The padded 16-bit tiles of NP planes of one filter block that share a geometry: luma (NP = 1, 64x64, pitch kTP),
+// or Cb and Cr (NP = 2, 32x32 each, pitch kTPC, the Cr tile kTileC elements after the Cb tile).  Tile origin (row 3,
+// col 8) = first pixel of the filter block; everything outside the copied rectangle is CDEF_VERY_LARGE
+// (cdef_process.c:211-230).  Only the (fbs + 6) x (fbs + 16) pixels the filter can read are written.  A thread moves
+// words of 8 pixels (one 8-byte load and PRMT widening at 8 bit, one 16-byte load at 16 bit, one 16-byte store), kLd
+// words' loads in flight before the first store.  A word starts at a multiple of 8 pixels in the plane; a plane
+// whose origin or pitch is not aligned to that, and a word the copied rectangle cuts, move pixel by pixel.
+template <typename PIX, int NP>
+__device__ void stage_cdef_tiles(uint16_t* tile, const PIX* plane0, const PIX* plane1, int stride, int fbr, int fbc, int nvfb, int nhfb,
+                                 int vsz, int hsz) {
+    constexpr int FBS = 64 / NP, TP = NP == 1 ? kTP : kTPC, WPR = (FBS + 16) / 8, PER = (FBS + 6) * WPR, kLd = 4;
     const int yoff = 3 * (fbr != 0), xoff = 8 * (fbc != 0);
     const int ysize = vsz + 3 * (fbr + 1 < nvfb) + yoff, xsize = hsz + 8 * (fbc + 1 < nhfb) + xoff;
-    const int py0 = fbr * fbs - yoff, px0 = fbc * fbs - xoff;
-    const int pairs = (fbs + 16) / 2;
-    // a pair starts at an even column: one load per pair when the plane's rows are aligned to it
-    const bool pair_load = (((size_t)plane | (size_t)stride * sizeof(PIX)) & (2 * sizeof(PIX) - 1)) == 0;
-#pragma unroll 4
-    for (int i = threadIdx.x; i < (fbs + 6) * pairs; i += blockDim.x) {
-        const int r = i / pairs, c = (i - r * pairs) * 2;
-        const int rr = r - (3 - yoff), cc = c - (8 - xoff);  // cc is even, xsize is a multiple of 4: the pair is in or out together
-        uint32_t v = (uint32_t)kVeryLarge * 0x10001u;
-        if (rr >= 0 && rr < ysize && cc >= 0 && cc < xsize) {
-            const PIX* p = plane + (size_t)(py0 + rr) * stride + px0 + cc;
-            if (!pair_load) v = (uint32_t)p[0] | ((uint32_t)p[1] << 16);
-            else if (sizeof(PIX) == 1) v = __byte_perm(*reinterpret_cast<const uint16_t*>(p), 0, 0x4140);  // 0, p[1], 0, p[0]
-            else v = *reinterpret_cast<const uint32_t*>(p);
+    const int py0 = fbr * FBS - yoff, px0 = fbc * FBS - xoff;
+    constexpr size_t kAl = 8 * sizeof(PIX) - 1;
+    const unsigned word = ((((size_t)plane0 | (size_t)stride * sizeof(PIX)) & kAl) == 0) |
+                          (((((size_t)plane1 | (size_t)stride * sizeof(PIX)) & kAl) == 0) << 1);
+    constexpr uint32_t kVL2 = (uint32_t)kVeryLarge * 0x10001u;
+    for (int i0 = threadIdx.x; i0 < NP * PER; i0 += kLd * kT2Threads) {
+        uint4 v[kLd];
+#pragma unroll
+        for (int k = 0; k < kLd; k++) {
+            const int i = i0 + k * kT2Threads, p = NP == 2 && i >= PER, q = i - p * PER;
+            const int r = q / WPR, c = (q - r * WPR) * 8;
+            const int rr = r - (3 - yoff), cc = c - (8 - xoff);
+            v[k] = make_uint4(kVL2, kVL2, kVL2, kVL2);
+            if (i < NP * PER && rr >= 0 && rr < ysize && cc + 8 > 0 && cc < xsize) {
+                const PIX* row = (p ? plane1 : plane0) + (size_t)(py0 + rr) * stride + px0;
+                if (((word >> p) & 1) && cc >= 0 && cc + 8 <= xsize) {
+                    v[k] = cdef_load_word8(row + cc);
+                } else {
+                    uint32_t e[8];
+#pragma unroll
+                    for (int j = 0; j < 8; j++) e[j] = cc + j >= 0 && cc + j < xsize ? (uint32_t)row[cc + j] : (uint32_t)kVeryLarge;
+                    v[k] = make_uint4(e[0] | e[1] << 16, e[2] | e[3] << 16, e[4] | e[5] << 16, e[6] | e[7] << 16);
+                }
+            }
         }
-        *reinterpret_cast<uint32_t*>(tile + r * kTP + c) = v;
+#pragma unroll
+        for (int k = 0; k < kLd; k++) {
+            const int i = i0 + k * kT2Threads, p = NP == 2 && i >= PER, q = i - p * PER;
+            const int r = q / WPR, c = (q - r * WPR) * 8;
+            if (i < NP * PER) *reinterpret_cast<uint4*>(tile + p * kTileC + r * TP + c) = v[k];
+        }
     }
     __syncthreads();
 }
@@ -374,55 +409,88 @@ struct CdefChunk {
     unsigned secs[2];      // per pass: bit c set when secondary code c (1..3) occurs
 };
 
-// Moments of one row segment (BS pixels at `in`, source at `o_row`) for every strength of `todo`, the
-// taps along one direction.  Luma (BS = 8) accumulates sum y, y^2, y*src; chroma (BS = 4) sum (src - y)^2.
-// Taps are loaded once per pixel and shared by all strengths; the primary half is recomputed only when the
-// primary strength changes and the secondary half once per distinct secondary code.
+// Moments of one row segment for every strength of `todo`, the taps along one direction.  Luma (BS = 8 pixels at
+// `in`, source at `o_row`) accumulates sum y, y^2, y*src into a0, a1, a2; chroma (BS = 4) sum (src - y)^2 of the Cb
+// row (`in`, `o_row`) into a0 and of the Cr row (`in2`, `o_row2`) into a1.  Two pixels are evaluated per step (luma:
+// two neighbours, chroma: the same pixel of both planes), so that their tap loads and strength chains interleave and
+// each strength's constants are read once for both.  Taps are loaded once per pixel and shared by all strengths; the
+// primary half is recomputed only when the primary strength changes and the secondary half once per distinct
+// secondary code.
 template <int BS, typename PIX>
-__device__ __forceinline__ void cdef_segment_pass(const uint16_t* in, const PIX* o_row, const int (&off)[6], const CdefChunk& C, int pass,
-                                                  const int (&tadj)[kGChunk], const uint4* tab, int cs, unsigned (&a0)[kGChunk],
-                                                  unsigned (&a1)[kGChunk], unsigned (&a2)[kGChunk]) {
+__device__ __forceinline__ void cdef_segment_pass(const uint16_t* in, const uint16_t* in2, const PIX* o_row, const PIX* o_row2,
+                                                  const int (&off)[6], const CdefChunk& C, int pass, const int (&tadj)[kGChunk],
+                                                  const uint4* tab, int cs, unsigned (&a0)[kGChunk], unsigned (&a1)[kGChunk],
+                                                  unsigned (&a2)[kGChunk]) {
     const unsigned todo = C.todo[pass], pnew = pass ? 0u : C.pri_new, secs = C.secs[pass];
+    constexpr int STEP = BS == 8 ? 2 : 1;
 #pragma unroll 1
-    for (int j = 0; j < BS; j++) {
-        const int      x = in[j];
-        const unsigned o = o_row[j];
-        CdefTaps       T;
-        cdef_load_taps(in + j, off, x, T);
-        int s1 = 0, s2 = 0, s3 = 0;  // secondary halves of codes 1, 2, 3 (strengths 1, 2, 4 << cs)
-        if (secs & 2) s1 = cdef_secondary_sum(T, tab[1 << cs]);
-        if (secs & 4) s2 = cdef_secondary_sum(T, tab[2 << cs]);
-        if (secs & 8) s3 = cdef_secondary_sum(T, tab[4 << cs]);
-        int psum = 0;
+    for (int j = 0; j < BS; j += STEP) {
+        const uint16_t* px[2] = {in + j, BS == 8 ? in + j + 1 : in2 + j};
+        int      x[2];
+        unsigned o[2];
+        CdefTaps T[2];
+#pragma unroll
+        for (int k = 0; k < 2; k++) {
+            x[k] = px[k][0];
+            o[k] = BS == 8 ? o_row[j + k] : (k ? o_row2[j] : o_row[j]);
+            cdef_load_taps(px[k], off, x[k], T[k]);
+        }
+        int s1[2] = {0, 0}, s2[2] = {0, 0}, s3[2] = {0, 0};  // secondary halves of codes 1, 2, 3 (strengths 1, 2, 4 << cs)
+        if (secs & 2) {
+            const uint4 c = tab[1 << cs];
+#pragma unroll
+            for (int k = 0; k < 2; k++) s1[k] = cdef_secondary_sum(T[k], c);
+        }
+        if (secs & 4) {
+            const uint4 c = tab[2 << cs];
+#pragma unroll
+            for (int k = 0; k < 2; k++) s2[k] = cdef_secondary_sum(T[k], c);
+        }
+        if (secs & 8) {
+            const uint4 c = tab[4 << cs];
+#pragma unroll
+            for (int k = 0; k < 2; k++) s3[k] = cdef_secondary_sum(T[k], c);
+        }
+        int psum[2] = {0, 0};
 #pragma unroll
         for (int gi = 0; gi < kGChunk; gi++) {
             if (!((todo >> gi) & 1)) continue;  // CTA-uniform
-            if ((pnew >> gi) & 1) psum = cdef_primary_sum(T, tab[tadj[gi]]);
-            const int sc = C.sv[gi] & 3, ssum = sc == 1 ? s1 : (sc == 2 ? s2 : (sc == 3 ? s3 : 0));
-            // code 0 leaves the pixel unchanged (sum = 0, and x lies inside [min, max] of its own neighbourhood)
-            const unsigned y = C.sv[gi] == 0 ? (unsigned)x : (unsigned)cdef_finish_px(T, x, psum + ssum);
-            if (BS == 8) {
-                a0[gi] += y;
-                a1[gi] += y * y;
-                a2[gi] += y * o;
-            } else {
-                const int e = (int)o - (int)y;
-                a0[gi] += (unsigned)(e * e);
+            if ((pnew >> gi) & 1) {
+                const uint4 c = tab[tadj[gi]];
+#pragma unroll
+                for (int k = 0; k < 2; k++) psum[k] = cdef_primary_sum(T[k], c);
+            }
+            const int sc = C.sv[gi] & 3;
+#pragma unroll
+            for (int k = 0; k < 2; k++) {
+                const int ssum = sc == 1 ? s1[k] : (sc == 2 ? s2[k] : (sc == 3 ? s3[k] : 0));
+                // code 0 leaves the pixel unchanged (sum = 0, and x lies inside [min, max] of its own neighbourhood)
+                const unsigned y = C.sv[gi] == 0 ? (unsigned)x[k] : (unsigned)cdef_finish_px(T[k], x[k], psum[k] + ssum);
+                if (BS == 8) {
+                    a0[gi] += y;
+                    a1[gi] += y * y;
+                    a2[gi] += y * o[k];
+                } else {
+                    const int e = (int)o[k] - (int)y;
+                    if (k == 0) a0[gi] += (unsigned)(e * e);
+                    else a1[gi] += (unsigned)(e * e);
+                }
             }
         }
     }
 }
 
-// The strength search of one (filter block, plane): every thread owns processed row segments (luma: one
-// 8-pixel row of an 8x8, chroma: one 4-pixel row of a 4x4), so tap offsets and strength constants are
-// built once per segment, and only the R threads of a block combine their moments, by shuffles.  Their
-// sums go to shared memory once per (block, strength); warps then turn them into distortions (luma: the
-// psy formula on the five moments) and sum them over the blocks.
+// The strength search of one filter block in luma (BS = 8) or in both chroma planes (BS = 4): every thread owns
+// processed row segments (luma: one 8-pixel row of an 8x8, chroma: one 4-pixel row of the 4x4 in Cb and the same
+// row in Cr), so tap offsets and strength constants are built once per segment, and only the R threads of a block
+// combine their moments, by shuffles.  Their sums go to shared memory once per (block, strength); warps then turn
+// them into distortions (luma: the psy formula on the five moments, chroma: Cb + Cr) and sum them over the blocks.
 template <int BS, typename PIX>
-__device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4* tab, const PIX* src, int sstride, const int* strengths,
-                                               int n_strengths, int count, int subs, int cs, int pli, const uint8_t* s_list,
+__device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4* tab, const PIX* src, const PIX* src2, int sstride,
+                                               const int* strengths, int n_strengths, int count, int subs, int cs, const uint8_t* s_list,
                                                const uint8_t* s_dir, const int* s_var, unsigned (*s_mom)[3][64], unsigned (*s_src)[64],
                                                unsigned long long* mse_fb) {
+    constexpr int TP = BS == 8 ? kTP : kTPC;
     const int R = BS / subs, nseg = count * R;  // processed rows per block (a power of two: R divides 32)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int g0 = 0; g0 < n_strengths; g0 += kGChunk) {
@@ -457,8 +525,9 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
             const bool live = s < nseg;
             const int  bi = live ? s / R : 0, r = live ? s - bi * R : 0;
             const int  b = s_list[bi], by = b >> 3, bx = b & 7, row = BS * by + r * subs;
-            const uint16_t* in    = tile + (3 + row) * kTP + 8 + BS * bx;
-            const PIX*      o_row = src + (size_t)row * sstride + BS * bx;
+            const uint16_t* in     = tile + (3 + row) * TP + 8 + BS * bx;
+            const PIX*      o_row  = src + (size_t)row * sstride + BS * bx;
+            const PIX*      o_row2 = BS == 4 ? src2 + (size_t)row * sstride + BS * bx : o_row;
             unsigned a0[kGChunk], a1[kGChunk], a2[kGChunk];
 #pragma unroll
             for (int gi = 0; gi < kGChunk; gi++) a0[gi] = a1[gi] = a2[gi] = 0;
@@ -471,12 +540,12 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
             }
             int off[6];
             if (C.todo[0]) {
-                cdef_tap_offsets(s_dir[b], kTP, off);
-                cdef_segment_pass<BS, PIX>(in, o_row, off, C, 0, tadj, tab, cs, a0, a1, a2);
+                cdef_tap_offsets(s_dir[b], TP, off);
+                cdef_segment_pass<BS, PIX>(in, in + kTileC, o_row, o_row2, off, C, 0, tadj, tab, cs, a0, a1, a2);
             }
             if (C.todo[1]) {
-                cdef_tap_offsets(0, kTP, off);
-                cdef_segment_pass<BS, PIX>(in, o_row, off, C, 1, tadj, tab, cs, a0, a1, a2);
+                cdef_tap_offsets(0, TP, off);
+                cdef_segment_pass<BS, PIX>(in, in + kTileC, o_row, o_row2, off, C, 1, tadj, tab, cs, a0, a1, a2);
             }
             const bool lead = live && r == 0;
 #pragma unroll
@@ -484,17 +553,13 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
                 if (!((tested >> gi) & 1)) continue;  // CTA-uniform
                 for (int sh = R >> 1; sh > 0; sh >>= 1) {
                     a0[gi] += __shfl_xor_sync(0xffffffffu, a0[gi], sh);
-                    if (BS == 8) {
-                        a1[gi] += __shfl_xor_sync(0xffffffffu, a1[gi], sh);
-                        a2[gi] += __shfl_xor_sync(0xffffffffu, a2[gi], sh);
-                    }
+                    a1[gi] += __shfl_xor_sync(0xffffffffu, a1[gi], sh);
+                    if (BS == 8) a2[gi] += __shfl_xor_sync(0xffffffffu, a2[gi], sh);
                 }
                 if (lead) {
                     s_mom[gi][0][bi] = a0[gi];
-                    if (BS == 8) {
-                        s_mom[gi][1][bi] = a1[gi];
-                        s_mom[gi][2][bi] = a2[gi];
-                    }
+                    s_mom[gi][1][bi] = a1[gi];
+                    if (BS == 8) s_mom[gi][2][bi] = a2[gi];
                 }
             }
             if (BS == 8 && g0 == 0) {  // the source's moments do not depend on the strength
@@ -519,71 +584,92 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
         // per strength: the blocks' distortions, summed by one warp
         for (int gi = warp; gi < ng; gi += kT2Threads / 32) {
             const int          sv = strengths[g0 + gi];
-            unsigned long long acc = 0;
+            unsigned long long acc = 0, acc2 = 0;  // luma; chroma: Cb, Cr
             if (sv >= 0)
-                for (int bi = lane; bi < count; bi += 32)
-                    acc += BS == 8 ? cdef_dist_from_sums(s_mom[gi][0][bi], s_src[0][bi], s_mom[gi][1][bi], s_src[1][bi], s_mom[gi][2][bi], cs)
-                                   : (unsigned long long)s_mom[gi][0][bi];
+                for (int bi = lane; bi < count; bi += 32) {
+                    if (BS == 8) {
+                        acc += cdef_dist_from_sums(s_mom[gi][0][bi], s_src[0][bi], s_mom[gi][1][bi], s_src[1][bi], s_mom[gi][2][bi], cs);
+                    } else {
+                        acc += s_mom[gi][0][bi];
+                        acc2 += s_mom[gi][1][bi];
+                    }
+                }
 #pragma unroll
-            for (int sh = 16; sh > 0; sh >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, sh);
+            for (int sh = 16; sh > 0; sh >>= 1) {
+                acc += __shfl_xor_sync(0xffffffffu, acc, sh);
+                if (BS == 4) acc2 += __shfl_xor_sync(0xffffffffu, acc2, sh);
+            }
             if (lane == 0) {
-                unsigned long long* m = mse_fb + g0 + gi;
-                // enc: mse_seg = (sum >> 2*coeff_shift) * subsampling_factor; untested chroma = default_mse_uv*64
-                const unsigned long long v = sv >= 0 ? (acc >> (2 * cs)) * (unsigned long long)subs : 0;
-                if (pli == 0) *m = v;
-                else atomicAdd(m, sv < 0 ? (pli == 1 ? 1040400ull * 64ull : 0ull) : v);
+                // enc: mse_seg = (sum >> 2*coeff_shift) * subsampling_factor per plane, Cb and Cr added; an untested
+                // chroma strength costs default_mse_uv*64 (once for both planes)
+                const unsigned long long v = ((acc >> (2 * cs)) + (BS == 4 ? acc2 >> (2 * cs) : 0ull)) * (unsigned long long)subs;
+                mse_fb[g0 + gi] = sv >= 0 ? v : (BS == 4 ? 1040400ull * 64ull : 0ull);
             }
         }
         __syncthreads();  // s_mom is reused by the next chunk
     }
 }
 
-// Strength search: one CTA per (filter block, plane).  mse[1] (chroma) must be zero on entry: the two
-// chroma planes add into it.
+// Work items of the search and apply grids: the chroma pair (Cb + Cr) of every filter block, then its luma.  A
+// chroma item is the longer one in the search, so it is handed out first.
+__device__ __forceinline__ bool cdef_item(int work, int nfb, int& fb) {
+    const bool chroma = work < nfb;
+    fb = chroma ? work : work - nfb;
+    return chroma;
+}
+
+// Strength search: one CTA per filter block and luma, and one per filter block and both chroma planes.  Every
+// mse[plane][fb][g] is written once.
 template <typename PIX>
 __global__ void __launch_bounds__(kT2Threads, 5)
 cdef_search_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const int* __restrict__ strengths_y,
                    const int* __restrict__ strengths_uv, int n_strengths, unsigned long long* __restrict__ mse /*[2][nfb][n_strengths]*/,
                    const uint8_t* __restrict__ dir_in /*[nfb][64]*/, const int* __restrict__ var_in /*[nfb][64]*/) {
-    __shared__ __align__(16) uint16_t tile[kTileRows * kTP];
-    __shared__ uint4    s_tab[2][256];  // cdef_strength_consts of every strength value, luma / chroma damping
+    __shared__ __align__(16) uint16_t tile[kTileRows * kTP];  // the luma tile, or the Cb and Cr tiles
+    __shared__ uint4    s_tab[256];  // cdef_strength_consts of every strength value at the damping of the item's planes
     __shared__ uint8_t  s_dir[64];
     __shared__ int      s_var[64];
     __shared__ uint8_t  s_list[64];
     __shared__ unsigned s_ballot[2];
-    __shared__ unsigned s_mom[kGChunk][3][64];  // per strength, per listed block: luma sum y, y^2, y*src; chroma [0] = sum (src - y)^2
+    __shared__ unsigned s_mom[kGChunk][3][64];  // per strength, per listed block: luma sum y, y^2, y*src; chroma sum (src - y)^2 of Cb, Cr
     __shared__ unsigned s_src[2][64];           // per listed luma block: sum src, src^2
     const int nhfb = (f.width + 63) >> 6, nvfb = (f.height + 63) >> 6, nfb = nhfb * nvfb;
     const int cs = f.bit_depth > 8 ? f.bit_depth - 8 : 0;
     const int w8 = (f.width + 7) >> 3, h8 = (f.height + 7) >> 3;
-    // strengths reach (15 << 4) = 240 (primary, 12-bit), adjusted ones no more, secondary 4 << 4
-    for (int i = threadIdx.x; i < 2 * 256; i += kT2Threads) s_tab[i >> 8][i & 255] = cdef_strength_consts(i & 255, f.damping + cs - (i >> 8), cs);
-    for (int work = blockIdx.x; work < nfb * 3; work += gridDim.x) {
-        const int fb = work / 3, pli = work - fb * 3;
-        const int fbr = fb / nhfb, fbc = fb - fbr * nhfb;
+    int tab_damping = -1;
+    for (int work = blockIdx.x; work < nfb * 2; work += gridDim.x) {
+        int        fb;
+        const bool chroma = cdef_item(work, nfb, fb);
+        const int  fbr = fb / nhfb, fbc = fb - fbr * nhfb;
+        const int  damping = f.damping + cs - chroma;
         __syncthreads();
+        if (damping != tab_damping) {  // CTA-uniform; cdef_fb_list's barrier publishes the table
+            // strengths reach (15 << 4) = 240 (primary, 12-bit), adjusted ones no more, secondary 4 << 4
+            for (int i = threadIdx.x; i < 256; i += kT2Threads) s_tab[i] = cdef_strength_consts(i, damping, cs);
+            tab_damping = damping;
+        }
         const int count = cdef_fb_list(skip8x8, dir_in, var_in, fb, fbr, fbc, w8, h8, s_list, s_dir, s_var, s_ballot);
+        unsigned long long* mse_fb = mse + (size_t)(chroma * nfb + fb) * n_strengths;
         if (count == 0) {
-            if (pli == 0)
-                for (int g = threadIdx.x; g < n_strengths; g += blockDim.x) mse[(size_t)fb * n_strengths + g] = 0;
+            for (int g = threadIdx.x; g < n_strengths; g += blockDim.x) mse_fb[g] = 0;
             continue;
         }
-        const int dec = pli ? 1 : 0;
-        const PIX* rec = (const PIX*)(pli == 0 ? f.recon_y : (pli == 1 ? f.recon_cb : f.recon_cr));
-        const PIX* src = (const PIX*)(pli == 0 ? f.src_y : (pli == 1 ? f.src_cb : f.src_cr));
-        const int rstride = pli ? f.recon_stride_c : f.recon_stride_y, sstride = pli ? f.src_stride_c : f.src_stride_y;
-        const int pw = f.width >> dec, ph = f.height >> dec, fbs = 64 >> dec;
-        const int hsz = min(fbs, pw - fbc * fbs), vsz = min(fbs, ph - fbr * fbs);
-        stage_cdef_tile<PIX>(tile, rec, rstride, fbr, fbc, nvfb, nhfb, fbs, vsz, hsz);  // ends with a barrier
-        const PIX* src_fb = src + (size_t)fbr * fbs * sstride + fbc * fbs;
-        unsigned long long* mse_fb = mse + (size_t)((pli ? 1 : 0) * nfb + fb) * n_strengths;
-        const int subs = min(f.subsampling_factor, dec ? 1 : 4);  // cdef_process.c:243-248 (4:2:0 chroma = BLOCK_4X4)
-        if (pli == 0)
-            cdef_search_fb<8, PIX>(tile, s_tab[0], src_fb, sstride, strengths_y, n_strengths, count, subs, cs, pli, s_list, s_dir, s_var,
-                                   s_mom, s_src, mse_fb);
-        else
-            cdef_search_fb<4, PIX>(tile, s_tab[1], src_fb, sstride, strengths_uv, n_strengths, count, subs, cs, pli, s_list, s_dir, s_var,
-                                   s_mom, s_src, mse_fb);
+        if (!chroma) {
+            const int hsz = min(64, f.width - fbc * 64), vsz = min(64, f.height - fbr * 64);
+            const PIX* rec = (const PIX*)f.recon_y;
+            stage_cdef_tiles<PIX, 1>(tile, rec, rec, f.recon_stride_y, fbr, fbc, nvfb, nhfb, vsz, hsz);  // ends with a barrier
+            const PIX* src_fb = (const PIX*)f.src_y + (size_t)fbr * 64 * f.src_stride_y + fbc * 64;
+            const int  subs = min(f.subsampling_factor, 4);  // cdef_process.c:243-248
+            cdef_search_fb<8, PIX>(tile, s_tab, src_fb, src_fb, f.src_stride_y, strengths_y, n_strengths, count, subs, cs, s_list, s_dir,
+                                   s_var, s_mom, s_src, mse_fb);
+        } else {
+            const int hsz = min(32, (f.width >> 1) - fbc * 32), vsz = min(32, (f.height >> 1) - fbr * 32);
+            stage_cdef_tiles<PIX, 2>(tile, (const PIX*)f.recon_cb, (const PIX*)f.recon_cr, f.recon_stride_c, fbr, fbc, nvfb, nhfb, vsz, hsz);
+            const size_t o = (size_t)fbr * 32 * f.src_stride_c + fbc * 32;
+            const int subs = min(f.subsampling_factor, 1);  // 4:2:0 chroma = BLOCK_4X4
+            cdef_search_fb<4, PIX>(tile, s_tab, (const PIX*)f.src_cb + o, (const PIX*)f.src_cr + o, f.src_stride_c, strengths_uv, n_strengths,
+                                   count, subs, cs, s_list, s_dir, s_var, s_mom, s_src, mse_fb);
+        }
     }
 }
 
@@ -609,38 +695,46 @@ __device__ __forceinline__ void cdef_store_row(PIX* p, const int (&y)[BS], bool 
     }
 }
 
-// the filter of one (filter block, plane) with one strength: a thread per BS-pixel row of a block
+// the filter of one filter block with one strength, in luma (BS = 8) or in both chroma planes (BS = 4, the Cr tile
+// kTileC elements after the Cb tile): a thread per BS-pixel row of a block, in every plane of the item
 template <int BS, typename PIX>
-__device__ __forceinline__ void cdef_apply_fb(const uint16_t* tile, PIX* out_fb, int ostride, bool wide, int count, int pri, int sec,
-                                              int damping, int cs, const uint8_t* s_list, const uint8_t* s_dir, const int* s_var) {
+__device__ __forceinline__ void cdef_apply_fb(const uint16_t* tile, PIX* out_fb, PIX* out_fb2, int ostride, unsigned wide, int count,
+                                              int pri, int sec, int damping, int cs, const uint8_t* s_list, const uint8_t* s_dir,
+                                              const int* s_var) {
+    constexpr int TP = BS == 8 ? kTP : kTPC, NP = BS == 8 ? 1 : 2;
     const uint4 csec = cdef_strength_consts(sec, damping, cs);
     for (int s = threadIdx.x; s < count * BS; s += kT2Threads) {
         const int bi = s / BS, r = s - bi * BS;
         const int b = s_list[bi], by = b >> 3, bx = b & 7;
         const uint4 cpri = cdef_strength_consts(BS == 4 ? pri : cdef_adjust_strength(pri, s_var[b]), damping, cs);
         int off[6];
-        cdef_tap_offsets(pri ? s_dir[b] : 0, kTP, off);
-        const uint16_t* in = tile + (3 + BS * by + r) * kTP + 8 + BS * bx;
-        int y[BS];
+        cdef_tap_offsets(pri ? s_dir[b] : 0, TP, off);
+        const uint16_t* in = tile + (3 + BS * by + r) * TP + 8 + BS * bx;
+        int y[NP][BS];
 #pragma unroll
-        for (int j = 0; j < BS; j++) {
-            CdefTaps  T;
-            const int x = in[j];
-            cdef_load_taps(in + j, off, x, T);
-            y[j] = cdef_finish_px(T, x, (pri ? cdef_primary_sum(T, cpri) : 0) + (sec ? cdef_secondary_sum(T, csec) : 0));
-        }
-        cdef_store_row<BS, PIX>(out_fb + (size_t)(BS * by + r) * ostride + BS * bx, y, wide);
+        for (int j = 0; j < BS; j++)
+#pragma unroll
+            for (int p = 0; p < NP; p++) {
+                CdefTaps  T;
+                const int x = in[p * kTileC + j];
+                cdef_load_taps(in + p * kTileC + j, off, x, T);
+                y[p][j] = cdef_finish_px(T, x, (pri ? cdef_primary_sum(T, cpri) : 0) + (sec ? cdef_secondary_sum(T, csec) : 0));
+            }
+        const size_t o = (size_t)(BS * by + r) * ostride + BS * bx;
+        cdef_store_row<BS, PIX>(out_fb + o, y[0], wide & 1);
+        if (NP == 2) cdef_store_row<BS, PIX>(out_fb2 + o, y[NP - 1], wide >> 1);
     }
 }
 
 // frame apply (svt_av1_cdef_frame, enc_cdef.c:284-600): per filter block strengths already chosen,
-// directions/variances as found by cdef_dir_kernel.  One CTA per (filter block, plane).
+// directions/variances as found by cdef_dir_kernel.  One CTA per filter block and luma, and one per filter block
+// and both chroma planes (they share one strength).
 template <typename PIX>
 __global__ void __launch_bounds__(kT2Threads)
 cdef_apply_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const int8_t* __restrict__ fb_strength_idx,
                   const int* __restrict__ y_strength, const int* __restrict__ uv_strength, const uint8_t* __restrict__ dir_in,
                   const int* __restrict__ var_in, PIX* out_y, PIX* out_cb, PIX* out_cr, int out_stride_y, int out_stride_c) {
-    __shared__ __align__(16) uint16_t tile[kTileRows * kTP];
+    __shared__ __align__(16) uint16_t tile[kTileRows * kTP];  // the luma tile, or the Cb and Cr tiles
     __shared__ uint8_t  s_dir[64];
     __shared__ int      s_var[64];
     __shared__ uint8_t  s_list[64];
@@ -648,12 +742,17 @@ cdef_apply_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const
     const int nhfb = (f.width + 63) >> 6, nvfb = (f.height + 63) >> 6, nfb = nhfb * nvfb;
     const int cs = f.bit_depth > 8 ? f.bit_depth - 8 : 0;
     const int w8 = (f.width + 7) >> 3, h8 = (f.height + 7) >> 3;
-    for (int work = blockIdx.x; work < nfb * 3; work += gridDim.x) {
-        const int fb = work / 3, pli = work - fb * 3;
-        const int fbr = fb / nhfb, fbc = fb - fbr * nhfb;
-        const int sidx = fb_strength_idx[fb];
+    // rows of a block start at multiples of its row within a picture row: one store per row when the plane is aligned to it
+    const auto wide_rows = [](const PIX* out, int ostride, size_t row_bytes) {
+        return (((size_t)out | (size_t)ostride * sizeof(PIX)) & (row_bytes - 1)) == 0;
+    };
+    for (int work = blockIdx.x; work < nfb * 2; work += gridDim.x) {
+        int        fb;
+        const bool chroma = cdef_item(work, nfb, fb);
+        const int  fbr = fb / nhfb, fbc = fb - fbr * nhfb;
+        const int  sidx = fb_strength_idx[fb];
         if (sidx < 0) continue;  // uniform per CTA
-        const int sv = pli ? uv_strength[sidx] : y_strength[sidx];
+        const int sv = chroma ? uv_strength[sidx] : y_strength[sidx];
         const int pri = (sv / 4) << cs;
         int sec = sv % 4;
         sec = (sec + (sec == 3)) << cs;
@@ -661,19 +760,21 @@ cdef_apply_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const
         __syncthreads();
         const int count = cdef_fb_list(skip8x8, dir_in, var_in, fb, fbr, fbc, w8, h8, s_list, s_dir, s_var, s_ballot);
         if (count == 0) continue;
-        const int dec = pli ? 1 : 0;
-        const PIX* rec = (const PIX*)(pli == 0 ? f.recon_y : (pli == 1 ? f.recon_cb : f.recon_cr));
-        PIX* out = pli == 0 ? out_y : (pli == 1 ? out_cb : out_cr);
-        const int rstride = pli ? f.recon_stride_c : f.recon_stride_y, ostride = pli ? out_stride_c : out_stride_y;
-        const int pw = f.width >> dec, ph = f.height >> dec, fbs = 64 >> dec;
-        const int hsz = min(fbs, pw - fbc * fbs), vsz = min(fbs, ph - fbr * fbs);
-        stage_cdef_tile<PIX>(tile, rec, rstride, fbr, fbc, nvfb, nhfb, fbs, vsz, hsz);  // ends with a barrier
-        PIX* out_fb = out + (size_t)fbr * fbs * ostride + fbc * fbs;
-        const int damping = f.damping + cs - (pli != 0);
-        const size_t row_bytes = (size_t)(8 >> dec) * sizeof(PIX);  // rows start at multiples of it within a picture row
-        const bool wide = (((size_t)out | (size_t)ostride * sizeof(PIX)) & (row_bytes - 1)) == 0;
-        if (pli == 0) cdef_apply_fb<8, PIX>(tile, out_fb, ostride, wide, count, pri, sec, damping, cs, s_list, s_dir, s_var);
-        else cdef_apply_fb<4, PIX>(tile, out_fb, ostride, wide, count, pri, sec, damping, cs, s_list, s_dir, s_var);
+        const int damping = f.damping + cs - chroma;
+        if (!chroma) {
+            const int hsz = min(64, f.width - fbc * 64), vsz = min(64, f.height - fbr * 64);
+            const PIX* rec = (const PIX*)f.recon_y;
+            stage_cdef_tiles<PIX, 1>(tile, rec, rec, f.recon_stride_y, fbr, fbc, nvfb, nhfb, vsz, hsz);  // ends with a barrier
+            PIX* out_fb = out_y + (size_t)fbr * 64 * out_stride_y + fbc * 64;
+            cdef_apply_fb<8, PIX>(tile, out_fb, out_fb, out_stride_y, wide_rows(out_y, out_stride_y, 8 * sizeof(PIX)), count, pri, sec,
+                                  damping, cs, s_list, s_dir, s_var);
+        } else {
+            const int hsz = min(32, (f.width >> 1) - fbc * 32), vsz = min(32, (f.height >> 1) - fbr * 32);
+            stage_cdef_tiles<PIX, 2>(tile, (const PIX*)f.recon_cb, (const PIX*)f.recon_cr, f.recon_stride_c, fbr, fbc, nvfb, nhfb, vsz, hsz);
+            const size_t o = (size_t)fbr * 32 * out_stride_c + fbc * 32;
+            const unsigned wide = wide_rows(out_cb, out_stride_c, 4 * sizeof(PIX)) | (wide_rows(out_cr, out_stride_c, 4 * sizeof(PIX)) << 1);
+            cdef_apply_fb<4, PIX>(tile, out_cb + o, out_cr + o, out_stride_c, wide, count, pri, sec, damping, cs, s_list, s_dir, s_var);
+        }
     }
 }
 
@@ -743,7 +844,7 @@ extern "C" void svt_b200_cdef_filter_block(uint8_t* dst8, uint16_t* dst16, int32
 extern "C" void svt_b200_aom_copy_rect8_8bit_to_16bit(uint16_t* dst, int32_t dstride, const uint8_t* src, int32_t sstride,
                                                       int32_t v, int32_t h) {
     // A widening host-to-host copy: the T2 path performs this conversion while staging the tile on
-    // the device (stage_cdef_tile); the T1 form has no device work to do.
+    // the device (stage_cdef_tiles); the T1 form has no device work to do.
     for (int i = 0; i < v; i++)
         for (int j = 0; j < h; j++) dst[i * dstride + j] = src[i * sstride + j];
 }
@@ -812,16 +913,15 @@ extern "C" int svt_b200_cdef_search_frame_dev(const SvtB200CdefFrame* frame, con
     const int nfb = ((frame->width + 63) >> 6) * ((frame->height + 63) >> 6);
     cudaStream_t st = (cudaStream_t)stream;
     const int nblk = ((frame->width + 7) >> 3) * ((frame->height + 7) >> 3);
-    B200_CUDA_CHECK(cudaMemsetAsync(d_mse + (size_t)nfb * n_strengths, 0, (size_t)nfb * n_strengths * sizeof(uint64_t), st));
     if (frame->bit_depth > 8) {
         cdef_dir_kernel<uint16_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, d_dir, d_var);
         B200_LAUNCH_CHECK();
-        cdef_search_kernel<uint16_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
+        cdef_search_kernel<uint16_t><<<grid_for((long long)nfb * 2, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
                                                                                 (unsigned long long*)d_mse, d_dir, d_var);
     } else {
         cdef_dir_kernel<uint8_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, d_dir, d_var);
         B200_LAUNCH_CHECK();
-        cdef_search_kernel<uint8_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
+        cdef_search_kernel<uint8_t><<<grid_for((long long)nfb * 2, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_strengths_y, d_strengths_uv, n_strengths,
                                                                                (unsigned long long*)d_mse, d_dir, d_var);
     }
     B200_LAUNCH_CHECK();
@@ -858,11 +958,11 @@ extern "C" int svt_b200_cdef_apply_frame_dev(const SvtB200CdefFrame* frame, cons
         d_var = g_cdef_var;
     }
     if (frame->bit_depth > 8)
-        cdef_apply_kernel<uint16_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
+        cdef_apply_kernel<uint16_t><<<grid_for((long long)nfb * 2, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
                                                                                d_dir, d_var, (uint16_t*)d_out_y, (uint16_t*)d_out_cb,
                                                                                (uint16_t*)d_out_cr, out_stride_y, out_stride_c);
     else
-        cdef_apply_kernel<uint8_t><<<grid_for((long long)nfb * 3, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
+        cdef_apply_kernel<uint8_t><<<grid_for((long long)nfb * 2, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
                                                                               d_dir, d_var, (uint8_t*)d_out_y, (uint8_t*)d_out_cb,
                                                                               (uint8_t*)d_out_cr, out_stride_y, out_stride_c);
     B200_LAUNCH_CHECK();
