@@ -601,6 +601,7 @@ typedef struct SvtB200WienerUnit {
     int16_t  hfilter[8];   /* WienerInfo.hfilter / vfilter: 7 taps + 0 */
     int16_t  vfilter[8];
 } SvtB200WienerUnit;
+/* bit_depth 8 (uint8 pixels), 10 or 12 (uint16); any other depth returns SVT_B200_ERR_BAD_ARG and launches nothing. */
 SVT_B200_API int svt_b200_wiener_units_dev(const void* d_src, void* d_dst, const SvtB200WienerUnit* d_units, int n_units,
                                            int bit_depth, void* stream);
 
@@ -613,7 +614,8 @@ typedef struct SvtB200StatsItem {
     int32_t  wiener_win;   /* 7, 5 or 3 */
     int32_t  reserved;
 } SvtB200StatsItem;
-/* d_M: [n_items][49], d_H: [n_items][49*49] (first win^2 resp. win^4 entries used, reference layout) */
+/* d_M: [n_items][49], d_H: [n_items][49*49] (first win^2 resp. win^4 entries used, reference layout).  bit_depth 8
+ * (uint8 pixels), 10 or 12 (uint16); any other depth returns SVT_B200_ERR_BAD_ARG and launches nothing. */
 SVT_B200_API int svt_b200_compute_stats_batch_dev(const void* d_dgd, const void* d_src, const SvtB200StatsItem* d_items,
                                                   int n_items, int bit_depth, int64_t* d_M, int64_t* d_H, void* stream);
 

@@ -496,6 +496,7 @@ extern "C" void svt_b200_av1_compute_stats_highbd(int32_t wiener_win, const uint
 extern "C" int svt_b200_wiener_units_dev(const void* d_src, void* d_dst, const SvtB200WienerUnit* d_units, int n_units, int bit_depth,
                                          void* stream) {
     require_ready();
+    if (bit_depth != 8 && bit_depth != 10 && bit_depth != 12) return SVT_B200_ERR_BAD_ARG;
     if (n_units <= 0) return n_units == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
     // get_conv_params_wiener (convolve.h): round_0 = 3 (+2 at 12 bit), round_1 = 2*FILTER_BITS - round_0
     const int round0 = bit_depth == 12 ? 5 : 3, round1 = 14 - round0;
@@ -511,8 +512,9 @@ extern "C" int svt_b200_wiener_units_dev(const void* d_src, void* d_dst, const S
 extern "C" int svt_b200_compute_stats_batch_dev(const void* d_dgd, const void* d_src, const SvtB200StatsItem* d_items, int n_items,
                                                 int bit_depth, int64_t* d_M, int64_t* d_H, void* stream) {
     require_ready();
+    if (bit_depth != 8 && bit_depth != 10 && bit_depth != 12) return SVT_B200_ERR_BAD_ARG;
     if (n_items <= 0) return n_items == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
-    if (bit_depth <= 8) {
+    if (bit_depth == 8) {
         launch_stats<uint8_t>((const uint8_t*)d_dgd, (const uint8_t*)d_src, d_items, n_items, 8, (long long*)d_M, (long long*)d_H, nullptr,
                               nullptr, (cudaStream_t)stream);
         return SVT_B200_OK;
