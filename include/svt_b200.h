@@ -798,6 +798,60 @@ SVT_B200_API int svt_b200_me_b64_num_pus(const SvtB200MeControls* ctrl);
 SVT_B200_API int svt_b200_me_b64_picture_dev(const SvtB200MePicture* cur, const SvtB200MePicture* refs, const SvtB200MeControls* ctrl,
                                              const SvtB200MeB64Results* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------ */
+/* K15 picture-analysis statistics  (reference: pic_analysis_process.c:166-1559)                */
+/* ------------------------------------------------------------------------------------------ */
+/* T1: aom_dsp_rtcd.h:858-862 (C: svt_compute_mean_c, svt_compute_mean_squared_values_c, svt_compute_sub_mean_8x8_c,
+ * svt_compute_interm_var_four8x8_c).  Each call sends only the rows it reads, so the caller's buffer may end at the last
+ * pixel read: (h - 1) * stride + w bytes for the first two, 6 * stride + 8 (sub mean) and 6 * stride + 32 (four 8x8) for
+ * the subsampled forms, which read rows 0, 2, 4 and 6. */
+SVT_B200_API uint64_t svt_b200_compute_mean_8x8(uint8_t* input_samples, uint32_t input_stride, uint32_t input_area_width,
+                                                uint32_t input_area_height);
+SVT_B200_API uint64_t svt_b200_compute_mean_square_values_8x8(uint8_t* input_samples, uint32_t input_stride, uint32_t input_area_width,
+                                                              uint32_t input_area_height);
+SVT_B200_API uint64_t svt_b200_compute_sub_mean_8x8(uint8_t* input_samples, uint16_t input_stride);
+SVT_B200_API void     svt_b200_compute_interm_var_four8x8(uint8_t* input_samples, uint16_t input_stride, uint64_t* mean_of8x8_blocks,
+                                                          uint64_t* mean_of_squared8x8_blocks);
+
+/* The SequenceControlSet fields svt_aom_gathering_picture_statistics (pic_analysis_process.c:1559) reads. */
+typedef struct SvtB200PaStatsControls {
+    int32_t calculate_variance;   /* scs->calculate_variance: the per-64x64 variances and pic_avg_variance */
+    int32_t block_mean_calc_prec; /* scs->block_mean_calc_prec: 0 = BLOCK_MEAN_PREC_FULL, 1 = BLOCK_MEAN_PREC_SUB (every other row) */
+    int32_t var_8x8;              /* static_config.enable_adaptive_quantization == 1 || static_config.variance_octile */
+    int32_t calc_hist;            /* scs->calc_hist: the region histograms, average intensities and avg_luma */
+    int32_t decim_step;           /* 1 or 4: static_config.scene_change_detection ? 1 : 4 */
+    int32_t regions_w, regions_h; /* picture_analysis_number_of_regions_per_width / _height, 1..4 */
+    int32_t reserved;
+} SvtB200PaStatsControls;
+#define SVT_B200_PA_MAX_REGIONS 4 /* MAX_NUMBER_OF_REGIONS_IN_WIDTH / _HEIGHT (pcs.h:42-43) */
+
+/* DEVICE buffers the call writes.  n_b64 = ceil(width / 64) * ceil(height / 64) of the full plane, raster order.
+ *   variance [n_b64][85] (me_context.h:54 order: 64x64 at 0, 32x32 at 1..4, 16x16 at 5..20, 8x8 at 21..84).  The reference
+ *            writes entries 1..84 only when var_8x8 is set and leaves them as they were otherwise; this call writes them as 0
+ *            then.  Not written when calculate_variance is 0.
+ *   pic_avg_variance  one uint16: mean of the 64x64 variances; 0 when calculate_variance is 0.
+ *   histogram [regions_w][regions_h][256], average_intensity [regions_w][regions_h]: not written when calc_hist is 0.
+ *   avg_luma  one uint64: the picture's mean luma over the 1/16 plane; INVALID_LUMA (256) when calc_hist is 0. */
+typedef struct SvtB200PaStatsResults {
+    uint16_t* variance;
+    uint16_t* pic_avg_variance;
+    uint32_t* histogram;
+    uint8_t*  average_intensity;
+    uint64_t* avg_luma;
+} SvtB200PaStatsResults;
+
+/* T2: svt_aom_gathering_picture_statistics for one picture.  The variances read plane[2] (full resolution), the histograms
+ * plane[0] (1/16 resolution, the reference's sixteenth_decimated_picture_ptr), interior only.  Like the reference, a 64x64
+ * block at the right or bottom edge is read whole: the full plane must have at least ceil64(width) - width columns of
+ * padding on the right (stride >= org_x + ceil64(width)) and ceil64(height) - height rows below, taken as org_y (the
+ * symmetric padding of an ME picture; the 72 of layout.ME_PAD covers any size).  Those pixels are read as they are, so the
+ * padding must hold what the reference's input_padded_pic holds: the replicated edge (svt_b200_extend_plane_dev).  The 1/16
+ * plane must be at least regions_w x regions_h and under 2^26 pixels.  Returns SVT_B200_ERR_BAD_ARG and launches nothing
+ * for a missing pointer, a plane that does not satisfy this, regions outside 1..4, decim_step other than 1 or 4 or an
+ * unknown precision; only the fields of the enabled parts are checked. */
+SVT_B200_API int svt_b200_picture_statistics_dev(const SvtB200MePicture* pic, const SvtB200PaStatsControls* ctl,
+                                                 const SvtB200PaStatsResults* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

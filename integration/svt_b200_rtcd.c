@@ -214,6 +214,12 @@ int svt_b200_install_rtcd(int device) {
     BIND(svt_aom_highbd_lpf_vertical_6, svt_b200_aom_highbd_lpf_vertical_6);
     BIND(svt_aom_highbd_lpf_vertical_8, svt_b200_aom_highbd_lpf_vertical_8);
     BIND(svt_aom_highbd_lpf_vertical_14, svt_b200_aom_highbd_lpf_vertical_14);
+    GROUP(512u);
+    /* K15: picture-analysis block means (aom_dsp_rtcd.h:858-862) */
+    BIND(svt_compute_mean_8x8, svt_b200_compute_mean_8x8);
+    BIND(svt_compute_mean_square_values_8x8, svt_b200_compute_mean_square_values_8x8);
+    BIND(svt_compute_sub_mean_8x8, svt_b200_compute_sub_mean_8x8);
+    BIND(svt_compute_interm_var_four8x8, svt_b200_compute_interm_var_four8x8);
     return SVT_B200_OK;
 }
 

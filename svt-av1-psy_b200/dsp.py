@@ -434,6 +434,38 @@ def me_picture_desc(planes, width, height):
         p.width[lvl] = w
         p.height[lvl] = h
     return p
+
+# ------------------------------------------------------------------------------------------------
+# K15 picture-analysis statistics
+# ------------------------------------------------------------------------------------------------
+for _n in ("svt_b200_compute_mean_8x8", "svt_b200_compute_mean_square_values_8x8"):
+    getattr(lib, _n).argtypes = [vp, ct.c_uint32, ct.c_uint32, ct.c_uint32]
+    getattr(lib, _n).restype = ct.c_uint64
+lib.svt_b200_compute_sub_mean_8x8.argtypes = [vp, ct.c_uint16]
+lib.svt_b200_compute_sub_mean_8x8.restype = ct.c_uint64
+lib.svt_b200_compute_interm_var_four8x8.argtypes = [vp, ct.c_uint16, vp, vp]
+lib.svt_b200_compute_interm_var_four8x8.restype = None
+lib.svt_b200_picture_statistics_dev.argtypes = [ct.POINTER(MePicture), ct.POINTER(PaStatsControls), ct.POINTER(PaStatsResults), vp]
+lib.svt_b200_picture_statistics_dev.restype = ct.c_int
+
+
+def picture_statistics_dev(pic, ctl, torch, stream=0):
+    """svt_b200_picture_statistics_dev on an ME picture (MePicture of device planes) with PaStatsControls `ctl`.  Returns
+    (rc, dict of the torch CUDA result tensors: variance [n_b64, 85] int16, pic_avg_variance [1] int16, histogram
+    [regions_w, regions_h, 256] int32, average_intensity [regions_w, regions_h] uint8, avg_luma [1] int64), all the bit
+    patterns of the C types.  Every array is pre-filled with 0xa5 bytes, so unwritten entries stay recognisable."""
+    n_b64 = ((pic.width[2] + 63) // 64) * ((pic.height[2] + 63) // 64)
+    rw, rh = max(int(ctl.regions_w), 1), max(int(ctl.regions_h), 1)
+    dev = torch.device("cuda")
+    out = {"variance": torch.full((n_b64, 85), -0x5a5b, dtype=torch.int16, device=dev),
+           "pic_avg_variance": torch.full((1,), -0x5a5b, dtype=torch.int16, device=dev),
+           "histogram": torch.full((rw, rh, 256), -0x5a5a5a5b, dtype=torch.int32, device=dev),
+           "average_intensity": torch.full((rw, rh), 0xa5, dtype=torch.uint8, device=dev),
+           "avg_luma": torch.full((1,), -0x5a5a5a5a5a5a5a5b, dtype=torch.int64, device=dev)}
+    res = PaStatsResults(*[out[n].data_ptr() for n, _ in PaStatsResults._fields_])
+    rc = lib.svt_b200_picture_statistics_dev(ct.byref(pic), ct.byref(ctl), ct.byref(res), vp(stream))
+    return rc, out
+
 lib.svt_b200_extend_plane_dev.argtypes = [vp, ct.c_int, ct.c_int, ct.c_int, ct.c_int, ct.c_int, vp]
 lib.svt_b200_extend_plane_dev.restype = ct.c_int
 lib.svt_b200_extend_planes_dev.argtypes = [ct.POINTER(PlaneExtent), ct.c_int, vp]

@@ -238,3 +238,13 @@ class MeB64Results(ct.Structure):  # device pointers
 # golden-fixture / comparison names of the ME outputs -> MeB64Results field (best_sad / best_mv are undefined for pruned references: not compared whole)
 ME_OUTPUT_NAMES = {"me_total": "total_me_candidate_index", "me_cand": "me_candidate_array", "me_mvs": "me_mv_array", "me_dist": "distortion",
                    "me_flags": "flags", "me_do_ref": "do_ref", "me_centre": "hme_centre", "me_zz": "zz_sad"}
+
+
+# ---- K15 picture-analysis statistics ----------------------------------------------------------------------------------
+class PaStatsControls(ct.Structure):
+    _fields_ = _same(ct.c_int32, "calculate_variance", "block_mean_calc_prec", "var_8x8", "calc_hist", "decim_step", "regions_w",
+                     "regions_h", "reserved")
+
+
+class PaStatsResults(ct.Structure):  # device pointers
+    _fields_ = _same(ct.c_void_p, "variance", "pic_avg_variance", "histogram", "average_intensity", "avg_luma")
