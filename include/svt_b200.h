@@ -655,6 +655,9 @@ typedef struct SvtB200SgrUnit {
     uint16_t params_idx; /* 0..15, svt_aom_eb_sgr_params */
     uint16_t reserved;
 } SvtB200SgrUnit;
+/* Every unit must fit within max_w x max_h (1 .. 128 each; they size the launch's shared memory).  bit_depth 8 (uint8
+ * pixels), 10 or 12 (uint16).  Any other depth, or max_w / max_h outside 1 .. 128, returns SVT_B200_ERR_BAD_ARG and
+ * launches nothing.  A filter whose radius is 0 leaves its output untouched. */
 SVT_B200_API int svt_b200_sgr_units_dev(const void* d_dgd, const SvtB200SgrUnit* d_units, int n_units, int32_t* d_flt0,
                                         int32_t* d_flt1, int bit_depth, int max_w, int max_h, void* stream);
 

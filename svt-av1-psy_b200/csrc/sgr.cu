@@ -291,8 +291,10 @@ extern "C" void svt_b200_get_proj_subspace(const uint8_t* src8, int width, int h
 extern "C" int svt_b200_sgr_units_dev(const void* d_dgd, const SvtB200SgrUnit* d_units, int n_units, int32_t* d_flt0, int32_t* d_flt1,
                                       int bit_depth, int max_w, int max_h, void* stream) {
     require_ready();
+    // the filter's rounding is defined for 8, 10 and 12 bit only; any other depth would run with the wrong one
+    if (bit_depth != 8 && bit_depth != 10 && bit_depth != 12) return SVT_B200_ERR_BAD_ARG;
+    if (max_w < 1 || max_h < 1 || max_w > 128 || max_h > 128) return SVT_B200_ERR_BAD_ARG;
     if (n_units <= 0) return n_units == 0 ? SVT_B200_OK : SVT_B200_ERR_BAD_ARG;
-    if (max_w > 128 || max_h > 128) return SVT_B200_ERR_BAD_ARG;
     if (bit_depth > 8) launch_sgr<uint16_t>((const uint16_t*)d_dgd, d_units, n_units, d_flt0, d_flt1, bit_depth, max_w, max_h, (cudaStream_t)stream);
     else launch_sgr<uint8_t>((const uint8_t*)d_dgd, d_units, n_units, d_flt0, d_flt1, 8, max_w, max_h, (cudaStream_t)stream);
     return SVT_B200_OK;

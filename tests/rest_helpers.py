@@ -95,6 +95,44 @@ def ref_selfguided(refc, dgd, off, w, h, stride, idx, bd):
     return f0, f1
 
 
+# svt_av1_selfguided_restoration_c keeps its 32-bit copy of the tile and its box sums in stack buffers of
+# RESTORATION_PROC_UNIT_PELS = (64 + 2 * 3 + 20)^2 elements (restoration.c:681,815,926)
+REF_PROC_UNIT_PELS = 90 * 90
+
+
+def ref_sgr_fits(w, h):
+    """whether the reference filter takes a w x h unit in one call: its box-sum rows are ((w + 6 + 3) & ~3) + 16 apart"""
+    return (h + 6) * ((((w + 6) + 3) & ~3) + 16) <= REF_PROC_UNIT_PELS and (w + 6) * (h + 6) <= REF_PROC_UNIT_PELS
+
+
+def ref_sgr_into(refc, dgd, off, w, h, stride, idx, bd, f0, f1, foff, fstride):
+    """svt_av1_selfguided_restoration_c of the w x h block at dgd[off] into f0 / f1 at element foff, rows fstride apart"""
+    assert ref_sgr_fits(w, h), (w, h)
+    f = refc.svt_av1_selfguided_restoration_c; f.restype = None
+    f(bptr(dgd, off), w, h, stride, P(f0, foff), P(f1, foff), fstride, idx, bd, int(dgd.dtype != np.uint8))
+
+
+def ref_sgr_tiled(refc, dgd, off, w, h, stride, idx, bd, f0, f1, foff, fstride, tw=64, rows=None):
+    """the reference filter of a unit of any size, as calls on sub-tiles at most tw wide whose bands start at `rows`
+    (default: every 64 rows).  The box sums of a sub-tile read the real neighbouring pixels, so this equals one call on
+    the whole unit as long as every band starts an even number of rows below the unit top: the r = 2 pass computes its
+    coefficients on every other row, counted from the top of the call."""
+    rows = list(range(0, h, 64)) if rows is None else list(rows)
+    for y0, y1 in zip(rows, rows[1:] + [h]):
+        for x0 in range(0, w, tw):
+            ref_sgr_into(refc, dgd, off + y0 * stride + x0, min(tw, w - x0), y1 - y0, stride, idx, bd, f0, f1, foff + y0 * fstride + x0,
+                         fstride)
+
+
+def decode_xq(xqd, prm):
+    """svt_decode_xq (restoration.c:634-645)"""
+    if prm[0] == 0:
+        return [0, 128 - xqd[1]]
+    if prm[1] == 0:
+        return [xqd[0], 0]
+    return [xqd[0], 128 - xqd[0] - xqd[1]]
+
+
 def port_selfguided(port, dgd16, off, w, h, stride, idx, bd):
     f0 = np.full(w * h, -12345, np.int32); f1 = np.full(w * h, -12345, np.int32)
     port.port_selfguided.restype = None

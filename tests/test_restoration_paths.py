@@ -43,9 +43,10 @@ def _device_view(torch, a, stride, skew):
     return flat, v
 
 
-def _run(b200, W, H, bd, us, skew, make_units, make_plane, want_fn):
+def _run(b200, W, H, bd, us, skew, make_units, make_plane, want_fn, frt=0, sse=False):
     """both boundary passes and the filter (normal and optimized_lr stripes) over three 4:2:0 planes; want_fn gives the
-    expected boundary lines (or None) and the expected restored plane per mode"""
+    expected boundary lines (or None) and the expected restored plane per mode.  frt is every plane's
+    frame_restoration_type; with sse, the unit SSE of each restored plane against its CDEF input is checked as well"""
     import torch
     planes = (b200.LrPlane * 3)()
     keep, checks = [], []
@@ -66,9 +67,10 @@ def _run(b200, W, H, bd, us, skew, make_units, make_plane, want_fn):
         d_bl = torch.full((2 * nst * bstride,), 77, dtype=tdt, device="cuda")
         d_units = torch.from_numpy(units.view(np.uint8)).cuda()
         planes[p] = b200.LrPlane(d_deb.data_ptr(), d_cdf.data_ptr(), d_dst.data_ptr(), d_cdf.data_ptr(), d_ab.data_ptr(), d_bl.data_ptr(), stride,
-                                 stride, stride, stride, bstride, w, h, ss, ss, usp, 0)
+                                 stride, stride, stride, bstride, w, h, ss, ss, usp, frt)
         assert d_cdf.data_ptr() % 16 == skew * d_cdf.element_size()
-        keep.append((k_deb, k_cdf, k_dst, d_dst, d_ab, d_bl, d_units))
+        d_sse = torch.full((hu * vu,), -1, dtype=torch.int64, device="cuda")
+        keep.append((k_deb, k_cdf, k_dst, d_dst, d_ab, d_bl, d_units, d_sse, cdf[PAD:PAD + h, PAD:PAD + w].astype(np.int64), (w, h, usp, hu, vu)))
         checks.append(want_fn(p, deb, cdf, w, h, ss, usp, units, nst, bstride))
     s = torch.cuda.current_stream().cuda_stream
     assert b200.lib.svt_b200_lr_save_boundary_lines_dev(planes, 3, 0, bd, s) == 0
@@ -80,15 +82,28 @@ def _run(b200, W, H, bd, us, skew, make_units, make_plane, want_fn):
             assert np.array_equal(keep[p][4].cpu().numpy().view(lines[0].dtype), lines[0]), ("above lines", p)
             assert np.array_equal(keep[p][5].cpu().numpy().view(lines[1].dtype), lines[1]), ("below lines", p)
     unit_ptrs = (ct.c_void_p * 3)(*[k[6].data_ptr() for k in keep])
+    sse_ptrs = (ct.c_void_p * 3)(*[k[7].data_ptr() for k in keep])
     for opt in (0, 1):
         for k in keep:
             k[3].zero_()
         assert b200.lib.svt_b200_lr_filter_frame_dev(planes, 3, unit_ptrs, opt, bd, s) == 0
+        if sse:
+            assert b200.lib.svt_b200_lr_unit_sse_dev(planes, 3, sse_ptrs, bd, s) == 0
         torch.cuda.synchronize()
         for p in range(3):
             want = checks[p][1][opt]
             got = keep[p][3].cpu().numpy().view(want.dtype)
             assert np.array_equal(got, want), ("restored plane", p, opt, np.argwhere(got != want)[:4])
+            if sse:  # sse_restoration_unit over each unit's limits, rows shifted up by the 8-row (luma) stripe offset
+                w, h, usp, hu, vu = keep[p][9]
+                d2 = (want.astype(np.int64) - keep[p][8]) ** 2
+                off = 8 >> (1 if p else 0)
+                got_sse = keep[p][7].cpu().numpy()
+                for ur in range(vu):
+                    vs, ve = max(0, ur * usp - off), (h if ur == vu - 1 else (ur + 1) * usp - off)
+                    for uc in range(hu):
+                        hs, he = uc * usp, (w if uc == hu - 1 else (uc + 1) * usp)
+                        assert int(got_sse[ur * hu + uc]) == int(d2[vs:ve, hs:he].sum()), ("unit sse", p, opt, ur, uc)
 
 
 def _reference(refc, W, H, bd):

@@ -53,11 +53,16 @@ print("RESULT " + json.dumps({"bytes": int(r), "packets": npk.value, "sha256": h
 '''
 
 
-def _encode(b200_on, **kw):
+def _encode(b200_on, groups=None, **kw):
+    """one encode in a fresh process; with b200_on the H100 tier is installed (only the kernel groups of the `groups` bit
+    mask, integration/svt_b200_rtcd.c, when it is given)"""
     env = dict(os.environ)
     env.pop("SVT_B200_DEVICE", None)
+    env.pop("SVT_B200_RTCD_GROUPS", None)
     if b200_on:
         env["SVT_B200_DEVICE"] = "0"
+        if groups is not None:
+            env["SVT_B200_RTCD_GROUPS"] = str(groups)
     code = _ENCODE % dict(kw, root=ROOT, lib=ENC_LIB, b200=os.path.join(ROOT, "svt-av1-psy_b200", "libsvtav1_b200.so"))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=1500)
     assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-3000:])
@@ -154,3 +159,26 @@ def test_encoder_bitstream_identical_to_c_path(cfg):
     assert g["launches"] > 10000, g  # the encode really ran on libsvtav1_b200.so
     assert (g["bytes"], g["packets"], g["sha256"]) == (c["bytes"], c["packets"], c["sha256"]), (c, g)
     print("encode %s: C %.1fs, H100 T1 pointers %.1fs, %d kernel launches" % (cfg, c["seconds"], g["seconds"], g["launches"]))
+
+
+# the preset-3 encodes: the `--asm c` half took 4.0 s (8 bit, lp = 8) and 9.7 s (10 bit, lp = 1) of encoder time on an
+# 8-core x86 host
+SGR_W, SGR_H, SGR_N = 640, 360, 4
+
+
+@pytest.mark.timeout(3000)
+# presets 0-3 are the ones that search self-guided restoration (SG level 3 and below); the 10-bit case pins lp = 1 for the
+# reason given above
+@pytest.mark.parametrize("cfg", [dict(w=SGR_W, h=SGR_H, n=SGR_N, bd=8, preset=3, crf=35, lp=8), dict(w=SGR_W, h=SGR_H, n=SGR_N, bd=10, preset=3, crf=35, lp=1)],
+                         ids=["8bit_M3", "10bit_M3_lp1"])
+def test_encoder_with_only_sgr_pointers_identical_to_c_path(cfg):
+    """with only the self-guided restoration pointers installed (kernel group 128: the filter, apply, both projection
+    errors and the projection subspace), the restoration search of a preset-3 encode calls them in its own shapes, and the
+    bitstream is the `--asm c` one"""
+    _need_lib()
+    c = _encode(False, **cfg)
+    g = _encode(True, groups=128, **cfg)
+    assert c["bytes"] > 0 and c["packets"] == cfg["n"], c
+    assert g["launches"] > 0, g  # the SGR pointers were called
+    assert (g["bytes"], g["packets"], g["sha256"]) == (c["bytes"], c["packets"], c["sha256"]), (c, g)
+    print("encode %s: C %.1fs, H100 SGR pointers %.1fs, %d kernel launches" % (cfg, c["seconds"], g["seconds"], g["launches"]))
