@@ -24,8 +24,6 @@
 // recomputed per strength.  The luma distortion's double-precision formula is evaluated with
 // round-to-nearest intrinsics in the reference's operand order (FMA contraction is disabled for the whole
 // library), which makes it IEEE-identical to the C code.
-#include <mutex>
-
 #include "common.cuh"
 #include "../../include/svt_b200.h"
 
@@ -928,12 +926,6 @@ extern "C" int svt_b200_cdef_search_frame_dev(const SvtB200CdefFrame* frame, con
     return SVT_B200_OK;
 }
 
-static uint8_t*   g_cdef_dir = nullptr;  // direction/variance scratch for apply calls that do not bring their own
-static int32_t*   g_cdef_var = nullptr;
-static size_t     g_cdef_cap = 0;
-static std::mutex g_cdef_mu;
-static ResetHook  g_cdef_reset([] { std::lock_guard<std::mutex> lk(g_cdef_mu); g_cdef_dir = nullptr; g_cdef_var = nullptr; g_cdef_cap = 0; });
-
 extern "C" int svt_b200_cdef_apply_frame_dev(const SvtB200CdefFrame* frame, const uint8_t* d_skip8x8, const int8_t* d_fb_strength_idx,
                                              const int* d_y_strength, const int* d_uv_strength, const uint8_t* d_dir,
                                              const int32_t* d_var, void* d_out_y, void* d_out_cb, void* d_out_cr, int out_stride_y,
@@ -943,19 +935,17 @@ extern "C" int svt_b200_cdef_apply_frame_dev(const SvtB200CdefFrame* frame, cons
     cudaStream_t st = (cudaStream_t)stream;
     const int nfb = ((frame->width + 63) >> 6) * ((frame->height + 63) >> 6);
     const int nblk = ((frame->width + 7) >> 3) * ((frame->height + 7) >> 3);
-    std::unique_lock<std::mutex> lk(g_cdef_mu, std::defer_lock);
-    if (!d_dir) {  // calls that share the scratch are serialised on the host (the stream orders the device side)
-        lk.lock();
-        if ((size_t)nfb > g_cdef_cap) {
-            g_cdef_cap = (size_t)nfb * 2;
-            g_cdef_dir = (uint8_t*)scratch_alloc(g_cdef_cap * 64);
-            g_cdef_var = (int32_t*)scratch_alloc(g_cdef_cap * 64 * 4);
-        }
-        if (frame->bit_depth > 8) cdef_dir_kernel<uint16_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, g_cdef_dir, g_cdef_var);
-        else cdef_dir_kernel<uint8_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, g_cdef_dir, g_cdef_var);
+    if (!d_dir) {  // the directions and variances the search would have given, in this stream's scratch
+        static char key;
+        const size_t dir_bytes = align256((size_t)nfb * 64);
+        uint8_t* sc = (uint8_t*)stream_scratch(&key, st, dir_bytes + (size_t)nfb * 64 * 4);
+        uint8_t* dir = sc;
+        int32_t* var = (int32_t*)(sc + dir_bytes);
+        if (frame->bit_depth > 8) cdef_dir_kernel<uint16_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, dir, var);
+        else cdef_dir_kernel<uint8_t><<<(nblk + 127) / 128, 128, 0, st>>>(*frame, d_skip8x8, dir, var);
         B200_LAUNCH_CHECK();
-        d_dir = g_cdef_dir;
-        d_var = g_cdef_var;
+        d_dir = dir;
+        d_var = var;
     }
     if (frame->bit_depth > 8)
         cdef_apply_kernel<uint16_t><<<grid_for((long long)nfb * 2, 16), kT2Threads, 0, st>>>(*frame, d_skip8x8, d_fb_strength_idx, d_y_strength, d_uv_strength,
@@ -966,6 +956,5 @@ extern "C" int svt_b200_cdef_apply_frame_dev(const SvtB200CdefFrame* frame, cons
                                                                               d_dir, d_var, (uint8_t*)d_out_y, (uint8_t*)d_out_cb,
                                                                               (uint8_t*)d_out_cr, out_stride_y, out_stride_c);
     B200_LAUNCH_CHECK();
-    if (lk.owns_lock()) B200_CUDA_CHECK(cudaStreamSynchronize(st));  // the scratch is free again when the call returns
     return SVT_B200_OK;
 }

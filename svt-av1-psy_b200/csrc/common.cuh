@@ -14,7 +14,10 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <mutex>
+#include <set>
+#include <utility>
 #include <vector>
 
 #define B200_CUDA_CHECK(expr)                                                                    \
@@ -48,9 +51,13 @@ struct Context {
     std::mutex          mu;
     std::vector<Lane*>  lanes;
     unsigned long long  launches = 0;  // kernels launched by this library (bench "gpu_launches")
-    // lifetime of module state (svt_b200_shutdown -> svt_b200_init on another device must not meet anything of the old one)
+    // device state of one initialisation: svt_b200_shutdown releases or forgets all of it, so that a later svt_b200_init
+    // (on the same or another device) meets nothing of the old one
+    struct StreamBuf { void* p = nullptr; size_t cap = 0; };
     int                          epoch = 0;      // bumped by every successful svt_b200_init
-    std::vector<void*>           scratch;        // every device scratch buffer of every module: freed at shutdown, never earlier
+    std::vector<void*>           scratch;        // every device scratch buffer ever taken: freed at shutdown, never earlier
+    std::map<std::pair<const void*, cudaStream_t>, StreamBuf> stream_bufs;  // stream_scratch(): current buffer per (key, stream)
+    std::set<const void*>        smem_opted_in;  // allow_dynamic_smem(): kernels whose attribute is set
     std::vector<cudaStream_t>    side_streams;   // ForkJoin handles of all host threads
     std::vector<cudaEvent_t>     side_events;
 };
@@ -60,12 +67,16 @@ void     require_ready();  // aborts loudly when svt_b200_init() has not succeed
 Lane*    lane_acquire();
 void     lane_release(Lane* l);
 void     count_launch(int n = 1);
-// Device scratch owned by the library.  A module that outgrows a buffer takes a new one and leaves the old one alone:
-// a CUDA graph captured earlier may still reference it.  Everything is released by svt_b200_shutdown().
-void*    scratch_alloc(size_t bytes);
-void     register_reset(void (*fn)());  // fn drops the module's cached scratch pointers / capacities (called at shutdown)
-int      epoch();                       // changes with every (re-)initialisation: per-function attributes are re-applied
-struct ResetHook { explicit ResetHook(void (*fn)()) { register_reset(fn); } };
+// Device scratch of at least `bytes` that belongs to one (key, stream).  `key` is any module-local address (a static tag),
+// so calls on different streams never share a buffer, and a call holds no lock across its launches.  A larger request
+// takes a new buffer of twice its size; the old one is neither freed nor moved before svt_b200_shutdown(), since a CUDA
+// graph captured earlier may still reference it.  A call that needs several arrays carves them at align256() offsets.
+void*    stream_scratch(const void* key, cudaStream_t stream, size_t bytes);
+static inline size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+// Lets `kernel` launch with `bytes` of dynamic shared memory (above the 48 KB default): the attribute is set by the first
+// call after each initialisation.
+void     allow_dynamic_smem(const void* kernel, size_t bytes);
+template <typename... A> void allow_dynamic_smem(void (*kernel)(A...), size_t bytes) { allow_dynamic_smem((const void*)kernel, bytes); }
 void     txfm_tables_init();  // txfm.cu: uploads the transform constant tables
 
 // Side streams for calls whose launches are independent of each other: fork_streams() makes the side

@@ -54,7 +54,7 @@ void RoundTrip::seal() {
         for (int i = 0; i < n_; i++) {
             Slot& s = slot_[i];
             if (s.kind != k) continue;
-            s.off = (end + 255) & ~size_t(255);
+            s.off = align256(end);
             end   = s.off + s.bytes;
             if ((k == kInOut || k == kOut) && d2h_off == ~size_t(0)) d2h_off = s.off;
         }
@@ -131,22 +131,22 @@ void lane_release(Lane* l) {
     l->busy = false;
 }
 
-void* scratch_alloc(size_t bytes) {
-    void* p = nullptr;
-    B200_CUDA_CHECK(cudaMalloc(&p, bytes ? bytes : 1));
+void* stream_scratch(const void* key, cudaStream_t stream, size_t bytes) {
     std::lock_guard<std::mutex> lk(g_ctx.mu);
-    g_ctx.scratch.push_back(p);
-    return p;
+    Context::StreamBuf& b = g_ctx.stream_bufs[{key, stream}];
+    if (bytes > b.cap) {
+        b.cap = bytes * 2;
+        B200_CUDA_CHECK(cudaMalloc(&b.p, b.cap));
+        g_ctx.scratch.push_back(b.p);
+    }
+    return b.p;
 }
-// the hooks register from static initialisers of other translation units: the list must not depend on the construction
-// order of namespace-scope objects, hence function-local statics
-static std::vector<void (*)()>& reset_list() { static std::vector<void (*)()> v; return v; }
-static std::mutex& reset_mu() { static std::mutex m; return m; }
-void register_reset(void (*fn)()) {
-    std::lock_guard<std::mutex> lk(reset_mu());
-    reset_list().push_back(fn);
+
+void allow_dynamic_smem(const void* kernel, size_t bytes) {
+    std::lock_guard<std::mutex> lk(g_ctx.mu);
+    if (g_ctx.smem_opted_in.insert(kernel).second)
+        B200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
 }
-int epoch() { return g_ctx.epoch; }
 
 void count_launch(int n) { __atomic_fetch_add(&g_ctx.launches, (unsigned long long)n, __ATOMIC_RELAXED); }
 
@@ -193,12 +193,10 @@ extern "C" void svt_b200_shutdown(void) {
     }
     c.lanes.clear();
     cudaDeviceSynchronize();
-    {
-        std::lock_guard<std::mutex> rl(reset_mu());
-        for (void (*fn)() : reset_list()) fn();   // modules forget their cached scratch / per-stream state ...
-    }
-    for (void* p : c.scratch) cudaFree(p);        // ... and the scratch itself goes (nothing was freed before: captured graphs)
+    for (void* p : c.scratch) cudaFree(p);  // nothing was freed before: captured graphs may have referenced any of it
     c.scratch.clear();
+    c.stream_bufs.clear();
+    c.smem_opted_in.clear();
     for (cudaStream_t s : c.side_streams) cudaStreamDestroy(s);
     for (cudaEvent_t e : c.side_events) cudaEventDestroy(e);
     c.side_streams.clear();

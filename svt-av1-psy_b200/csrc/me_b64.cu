@@ -25,8 +25,6 @@
 //                Writes one full-pel item per (reference, block) + the 85 SADs of the variance probe ("seed").
 //            (B) fullpel_search_kernel<TMA> (me_pyramid.cu) over the items, best arrays seeded with the probe.
 //            (C) me_b64_finish_kernel  one CTA per block: ME-based pruning, candidates, distortions, GM flags.
-#include <map>
-
 #include "common.cuh"
 #include "sad_small.cuh"
 #include "../../include/svt_b200.h"
@@ -882,16 +880,6 @@ me_b64_finish_kernel(const __grid_constant__ SvtB200MeControls c, int n_b64, int
     }
 }
 
-struct MeB64Workspace {
-    size_t cap = 0;  // (reference, block) pairs
-    SvtB200FullpelItem* items = nullptr;
-    uint32_t* seed = nullptr;
-    uint8_t*  do_ref = nullptr;
-};
-std::map<cudaStream_t, MeB64Workspace> g_ws;
-std::mutex g_mu;
-ResetHook g_reset([] { std::lock_guard<std::mutex> lk(g_mu); g_ws.clear(); });
-
 }  // namespace
 }  // namespace b200
 
@@ -926,28 +914,24 @@ extern "C" int svt_b200_me_b64_picture_dev(const SvtB200MePicture* cur, const Sv
     if (c.n_list < 2) tab.c.n_ref[1] = 0;
     for (int r = 0; r < c.n_ref[0]; r++) tab.ref[0][r] = refs[r];
     for (int r = 0; r < n1; r++) tab.ref[1][r] = refs[c.n_ref[0] + r];
-    MeB64Workspace* w;
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        w = &g_ws[st];
-        if ((size_t)pairs > w->cap) {  // new buffers; the old ones stay alive for graphs captured earlier (freed at shutdown)
-            w->cap = (size_t)pairs * 2;
-            w->items = (SvtB200FullpelItem*)scratch_alloc(w->cap * sizeof(SvtB200FullpelItem));
-            w->seed = (uint32_t*)scratch_alloc(w->cap * 85 * sizeof(uint32_t));
-            w->do_ref = (uint8_t*)scratch_alloc(w->cap * 8);
-        }
-    }
+    // this stream's workspace: a full-pel item and the 85 probe SADs per (reference, block) pair, each block's 8 do_ref flags
+    static char key;
+    const size_t items_bytes = align256((size_t)pairs * sizeof(SvtB200FullpelItem)), seed_bytes = align256((size_t)pairs * 85 * sizeof(uint32_t));
+    uint8_t* ws = (uint8_t*)stream_scratch(&key, st, items_bytes + seed_bytes + (size_t)pairs * 8);
+    SvtB200FullpelItem* items = (SvtB200FullpelItem*)ws;
+    uint32_t* seed = (uint32_t*)(ws + items_bytes);
+    uint8_t* do_ref = ws + items_bytes + seed_bytes;
     // the candidate / MV arrays are only partially written by design (me_sb_results_ctor leaves them uninitialised): defined zeros here
     B200_CUDA_CHECK(cudaMemsetAsync(out->total_me_candidate_index, 0, (size_t)n_b64 * n_pu, st));
     B200_CUDA_CHECK(cudaMemsetAsync(out->me_candidate_array, 0, (size_t)n_b64 * n_pu * c.max_cand, st));
     B200_CUDA_CHECK(cudaMemsetAsync(out->me_mv_array, 0, (size_t)n_b64 * n_pu * c.max_refs * 4, st));
-    me_b64_hme_kernel<<<n_b64, kHmeThreads, 0, st>>>(tab, n_b64, b64_w, w->items, w->seed, w->do_ref, out->hme_centre, out->zz_sad);
+    me_b64_hme_kernel<<<n_b64, kHmeThreads, 0, st>>>(tab, n_b64, b64_w, items, seed, do_ref, out->hme_centre, out->zz_sad);
     B200_LAUNCH_CHECK();
-    if (!launch_fullpel_tma(cur, refs, n_refs, n_b64, w->items, pairs, out->best_sad, out->best_mv, st, w->seed)) {
+    if (!launch_fullpel_tma(cur, refs, n_refs, n_b64, items, pairs, out->best_sad, out->best_mv, st, seed)) {
         fprintf(stderr, "[svt_b200] svt_b200_me_b64_picture_dev: the luma planes do not meet the layout rule (16-byte aligned base and pitch)\n");
         return SVT_B200_ERR_BAD_ARG;
     }
-    me_b64_finish_kernel<<<n_b64, 96, 0, st>>>(tab.c, n_b64, b64_w, W, H, n_pu, out->best_sad, out->best_mv, w->do_ref, out->total_me_candidate_index,
+    me_b64_finish_kernel<<<n_b64, 96, 0, st>>>(tab.c, n_b64, b64_w, W, H, n_pu, out->best_sad, out->best_mv, do_ref, out->total_me_candidate_index,
                                                 out->me_candidate_array, out->me_mv_array, out->distortion, out->flags, out->do_ref);
     B200_LAUNCH_CHECK();
     return SVT_B200_OK;

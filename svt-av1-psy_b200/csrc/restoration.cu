@@ -352,19 +352,8 @@ extern "C" int svt_b200_lr_filter_frame_dev(const SvtB200LrPlane* planes, int n_
         const LrGeom g = lr_geom(planes[i]);
         n_tiles += g.n_stripes * g.n_chunks;
     }
-    static std::mutex mu;
-    static bool attr8 = false, attr16 = false;
-    static int  attr_epoch = -1;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        if (attr_epoch != epoch()) { attr8 = attr16 = false; attr_epoch = epoch(); }
-        bool& a = bit_depth == 8 ? attr8 : attr16;
-        if (!a) {
-            if (bit_depth == 8) B200_CUDA_CHECK(cudaFuncSetAttribute(lr_filter_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLrSmem));
-            else B200_CUDA_CHECK(cudaFuncSetAttribute(lr_filter_kernel<uint16_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLrSmem));
-            a = true;
-        }
-    }
+    if (bit_depth == 8) allow_dynamic_smem(lr_filter_kernel<uint8_t>, kLrSmem);
+    else allow_dynamic_smem(lr_filter_kernel<uint16_t>, kLrSmem);
     // planes whose frame_restoration_type rules the self-guided filter out need only the Wiener footprint (more CTAs per SM)
     bool sgr_possible = false;
     for (int i = 0; i < n_planes; i++) sgr_possible |= planes[i].frame_restoration_type != 1;

@@ -290,17 +290,7 @@ void launch_sad_search(const uint8_t* d_src, const uint8_t* d_ref, const SvtB200
     const size_t dyn_max = (size_t)c.max_smem - 2048;  // opt-in limit minus this kernel's static shared memory
     if (smem > dyn_max) smem = dyn_max;
     if (smem < 32 * 1024) smem = 32 * 1024;
-    static std::mutex attr_mu;
-    static size_t     attr_set = 0;
-    static int        attr_epoch = -1;
-    {
-        std::lock_guard<std::mutex> lk(attr_mu);
-        if (attr_epoch != epoch()) { attr_set = 0; attr_epoch = epoch(); }  // re-initialised (possibly on another device): apply again
-        if (smem > attr_set) {
-            B200_CUDA_CHECK(cudaFuncSetAttribute(sad_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_max));
-            attr_set = dyn_max;
-        }
-    }
+    allow_dynamic_smem(sad_search_kernel, dyn_max);
     int ctas_per_sm = (int)(dyn_max / (smem + 1024));
     if (ctas_per_sm < 1) ctas_per_sm = 1;
     if (ctas_per_sm > 8) ctas_per_sm = 8;

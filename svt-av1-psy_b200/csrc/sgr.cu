@@ -152,18 +152,7 @@ template <typename PIX>
 static void launch_sgr(const PIX* d_dgd, const SvtB200SgrUnit* d_units, int n, int32_t* d_f0, int32_t* d_f1, int bd, int max_w, int max_h,
                        cudaStream_t st) {
     const size_t smem = sgr_smem(max_w, max_h);
-    static std::mutex mu;
-    static size_t set8 = 0, set16 = 0;
-    static int    set_epoch = -1;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        if (set_epoch != epoch()) { set8 = set16 = 0; set_epoch = epoch(); }
-        size_t& s = sizeof(PIX) == 1 ? set8 : set16;
-        if (smem > 48 * 1024 && smem > s) {
-            B200_CUDA_CHECK(cudaFuncSetAttribute(sgr_filter_kernel<PIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(ctx().max_smem - 1024)));
-            s = ctx().max_smem;
-        }
-    }
+    if (smem > 48 * 1024) allow_dynamic_smem(sgr_filter_kernel<PIX>, ctx().max_smem - 1024);
     sgr_filter_kernel<PIX><<<grid_for(n, 2), 256, smem, st>>>(d_dgd, d_units, n, d_f0, d_f1, bd);
     B200_LAUNCH_CHECK();
 }

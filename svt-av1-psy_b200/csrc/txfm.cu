@@ -14,8 +14,6 @@
 // 32- and 64-point vectors run split across two lanes.  The block sits in shared memory in element-major order with
 // an odd pitch, so the passes and the transposing hand-over are bank-conflict free; pixel, residual and coefficient
 // rows move between global memory and the planes in 4- to 16-byte words where the item's origin and stride allow it.
-#include <map>
-#include <mutex>
 #include <type_traits>
 #include <utility>
 #include "txfm_tables.cuh"
@@ -720,20 +718,9 @@ extern "C" int svt_b200_pack_levels_dev(const int32_t* d_qcoeff, const int16_t* 
     require_ready();
     if (n_items <= 0 || !d_offsets || !d_levels || !d_iscan || (level_bytes != 2 && level_bytes != 4)) return SVT_B200_ERR_BAD_ARG;
     const int chunks = (n_items + kPackChunk - 1) / kPackChunk;
-    if (chunks > 4096) return SVT_B200_ERR_BAD_ARG;  // the chunk sums live in the tail of the offsets buffer's lane scratch
-    static std::mutex mu;
-    static std::map<cudaStream_t, uint32_t*> sums_of;  // per-stream scratch: concurrent frames on different streams do not share it
-    uint32_t* d_sums;
-    {
-        std::lock_guard<std::mutex> lk(mu);
-        auto it = sums_of.find((cudaStream_t)stream);
-        static ResetHook hook([] { sums_of.clear(); });
-        if (it == sums_of.end()) {
-            d_sums = (uint32_t*)scratch_alloc(4096 * sizeof(uint32_t));
-            sums_of[(cudaStream_t)stream] = d_sums;
-        } else
-            d_sums = it->second;
-    }
+    if (chunks > 4096) return SVT_B200_ERR_BAD_ARG;  // the chunk sums' scratch holds 4096
+    static char key;  // the chunk sums, in this stream's scratch
+    uint32_t* d_sums = (uint32_t*)stream_scratch(&key, (cudaStream_t)stream, 4096 * sizeof(uint32_t));
     eob_chunk_sum_kernel<<<chunks, 256, 0, (cudaStream_t)stream>>>(d_eobs, n_items, d_sums, d_offsets);
     B200_LAUNCH_CHECK();
     eob_offsets_kernel<<<chunks, kPackChunk, 0, (cudaStream_t)stream>>>(d_eobs, d_sums, d_offsets, n_items);

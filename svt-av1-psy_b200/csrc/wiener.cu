@@ -15,8 +15,6 @@
 //   10/12-bit    -> the lag-sum kernels of wiener_stats_lag.cuh (H[p][q] depends only on the lag between the two samples).
 #include <cooperative_groups.h>
 
-#include <map>
-
 #include "common.cuh"
 #include "wiener_unit.cuh"
 #include "../../include/svt_b200.h"
@@ -367,27 +365,11 @@ stats_imma_kernel(const uint8_t* __restrict__ dgd_base, const uint8_t* __restric
     cluster.sync();  // no CTA leaves while another may still read its shared memory
 }
 
-// scratch of the 10/12-bit batch call (lag sums, pixel totals), one per stream: calls enqueued on
-// different streams may execute concurrently
-struct StatsScratch {
-    long long*          acc = nullptr;
-    unsigned long long* tot = nullptr;
-    size_t              cap = 0;
-};
-static std::map<cudaStream_t, StatsScratch> g_stats;
-static std::mutex g_stats_mu;
-static ResetHook g_stats_reset([] { std::lock_guard<std::mutex> lk(g_stats_mu); g_stats.clear(); });
-
 template <typename PIX, int WIN>
 static void launch_lag_bulk(const PIX* d_dgd, const PIX* d_src, const SvtB200StatsItem* d_items, int n, int cpi, unsigned long long* acc,
                             cudaStream_t st) {
     constexpr size_t smem = lag_bulk_smem<PIX, WIN>();
-    static int attr = -1;
-    if (attr != epoch()) {
-        if (smem > 48 * 1024)
-            B200_CUDA_CHECK(cudaFuncSetAttribute(stats_lag_bulk_kernel<PIX, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = epoch();
-    }
+    if (smem > 48 * 1024) allow_dynamic_smem(stats_lag_bulk_kernel<PIX, WIN>, smem);
     stats_lag_bulk_kernel<PIX, WIN><<<dim3(cpi, n), 256, smem, st>>>(d_dgd, d_src, d_items, acc);
     B200_LAUNCH_CHECK();
 }
@@ -519,14 +501,11 @@ extern "C" int svt_b200_compute_stats_batch_dev(const void* d_dgd, const void* d
                               nullptr, (cudaStream_t)stream);
         return SVT_B200_OK;
     }
-    std::lock_guard<std::mutex> lk(g_stats_mu);
-    StatsScratch& sc = g_stats[(cudaStream_t)stream];
-    if ((size_t)n_items > sc.cap) {
-        sc.cap = (size_t)n_items * 2;  // new buffers; the old ones live on until shutdown (captured graphs may replay them)
-        sc.acc = (long long*)scratch_alloc(sc.cap * kLagItemWords * 8);
-        sc.tot = (unsigned long long*)scratch_alloc(sc.cap * 8);
-    }
+    // the lag sums and pixel totals, in this stream's scratch
+    static char key;
+    const size_t acc_bytes = align256((size_t)n_items * kLagItemWords * 8);
+    uint8_t* sc = (uint8_t*)stream_scratch(&key, (cudaStream_t)stream, acc_bytes + (size_t)n_items * 8);
     launch_stats<uint16_t>((const uint16_t*)d_dgd, (const uint16_t*)d_src, d_items, n_items, bit_depth, (long long*)d_M, (long long*)d_H,
-                           sc.acc, sc.tot, (cudaStream_t)stream);
+                           (long long*)sc, (unsigned long long*)(sc + acc_bytes), (cudaStream_t)stream);
     return SVT_B200_OK;
 }
