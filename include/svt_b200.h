@@ -213,7 +213,7 @@ typedef struct SvtB200InvTxfmItem {
     uint32_t recon_stride;
     uint8_t  tx_size;
     uint8_t  tx_type;
-    uint8_t  bd;
+    uint8_t  bd;         /* 8, 10 or 12; a call on 1-byte pixels is the 8-bit path and takes bd as 8 */
     uint8_t  reserved;
     uint32_t reserved2;
 } SvtB200InvTxfmItem;

@@ -4,7 +4,9 @@
 // Reference behaviour restated: av1_tranform_two_d_core_c (Source/Lib/Codec/transforms.c:2259-2324)
 // and inv_txfm2d_add_c (Source/Lib/Codec/inv_transforms.c:2459-2534), for all 19 transform sizes and
 // 16 transform types, 8/10/12-bit.  The 2-D configuration table (flips, per-pass kernel, cos_bit,
-// shifts) is dumped from the reference (txfm_cfg.inc); the 1-D networks are txfm_graphs.inc.
+// shifts) is dumped from the reference (txfm_cfg.inc); the 1-D networks are txfm_graphs.inc.  The cosine bits and
+// stage shifts depend on the size alone and are compile-time constants of each size body (kTxSizeCfg); the flips and
+// the 1-D kernel types depend on the transform type and are read per item.
 //
 // H100 mapping: one kernel, txfm_kernel, whose modes are the forward batch, the inverse batch and the fused chain.
 // A transform block belongs to a team sized by its team class, log2(max(W,H)) - 2.  In the 4-, 8- and 16-point
@@ -22,23 +24,62 @@
 
 namespace b200 {
 
+// The constants of a 2-D transform that depend on its size alone: the forward's column and row cosine bits and its three
+// stage shifts, the inverse's two stage shifts (all as TxCfg holds them); the inverse's cosine bit is kInvCosBit at every
+// size.  They are compile-time constants of each size body, so the networks' weights and every rounding shift become
+// instruction immediates.  txfm_tables_init checks them against the table dumped from the reference for every valid
+// (size, type).
+struct TxSizeCfg {
+    int8_t f_cbc, f_cbr, f_s0, f_s1, f_s2, i_s0, i_s1;
+};
+constexpr int       kInvCosBit = 12;
+constexpr TxSizeCfg kTxSizeCfg[19] = {
+    {13, 13, 2, 0, 0, 0, -4},    // 0: 4x4
+    {13, 13, 2, -1, 0, -1, -4},  // 1: 8x8
+    {13, 12, 2, -2, 0, -2, -4},  // 2: 16x16
+    {12, 12, 2, -4, 0, -2, -4},  // 3: 32x32
+    {13, 10, 0, -2, -2, -2, -4}, // 4: 64x64
+    {13, 13, 2, -1, 0, 0, -4},   // 5: 4x8
+    {13, 13, 2, -1, 0, 0, -4},   // 6: 8x4
+    {13, 13, 2, -2, 0, -1, -4},  // 7: 8x16
+    {13, 13, 2, -2, 0, -1, -4},  // 8: 16x8
+    {12, 13, 2, -4, 0, -1, -4},  // 9: 16x32
+    {13, 13, 2, -4, 0, -1, -4},  // 10: 32x16
+    {13, 11, 0, -2, -2, -1, -4}, // 11: 32x64
+    {12, 11, 2, -4, -2, -1, -4}, // 12: 64x32
+    {13, 12, 2, -1, 0, -1, -4},  // 13: 4x16
+    {13, 13, 2, -1, 0, -1, -4},  // 14: 16x4
+    {12, 12, 2, -2, 0, -2, -4},  // 15: 8x32
+    {13, 12, 2, -2, 0, -2, -4},  // 16: 32x8
+    {13, 12, 0, -2, 0, -2, -4},  // 17: 16x64
+    {13, 12, 2, -4, 0, -2, -4},  // 18: 64x16
+};
+
 static TxCfg h_txcfg[19][16];
 const TxCfg& host_txcfg(int size, int type) { return h_txcfg[size][type]; }
 
 void txfm_tables_init() {
     memset(h_txcfg, 0, sizeof(h_txcfg));
-    static int32_t cosv[7][64], sinv[7][5];
 #define TXC(sz, ty, v, fud, flr, fs0, fs1, fs2, fcbc, fcbr, ftc, ftr, iud, ilr, is0, is1, icbc, icbr, itc, itr) \
     h_txcfg[sz][ty] = TxCfg{v, fud, flr, fs0, fs1, fs2, fcbc, fcbr, ftc, ftr, iud, ilr, is0, is1, icbc, icbr, itc, itr};
-#define TXCOS(bit, ...) { const int32_t t[64] = {__VA_ARGS__}; memcpy(cosv[bit - 10], t, sizeof(t)); }
-#define TXSIN(bit, ...) { const int32_t t[5] = {__VA_ARGS__}; memcpy(sinv[bit - 10], t, sizeof(t)); }
+#define TXCOS(...)
+#define TXSIN(...)
 #include "txfm_cfg.inc"
 #undef TXC
 #undef TXCOS
 #undef TXSIN
+    for (int sz = 0; sz < 19; sz++)
+        for (int ty = 0; ty < 16; ty++) {
+            const TxCfg& c = h_txcfg[sz][ty];
+            const TxSizeCfg& k = kTxSizeCfg[sz];
+            if (c.valid && (c.f_cbc != k.f_cbc || c.f_cbr != k.f_cbr || c.f_s0 != k.f_s0 || c.f_s1 != k.f_s1 || c.f_s2 != k.f_s2 ||
+                            c.i_s0 != k.i_s0 || c.i_s1 != k.i_s1 || c.i_cbc != kInvCosBit || c.i_cbr != kInvCosBit)) {
+                fprintf(stderr, "[svt_b200] FATAL %s:%d: the compile-time transform constants of tx_size %d differ from the "
+                                "reference's table at tx_type %d\n", __FILE__, __LINE__, sz, ty);
+                abort();
+            }
+        }
     B200_CUDA_CHECK(cudaMemcpyToSymbol(c_txcfg, h_txcfg, sizeof(h_txcfg)));
-    B200_CUDA_CHECK(cudaMemcpyToSymbol(c_cospi, cosv, sizeof(cosv)));
-    B200_CUDA_CHECK(cudaMemcpyToSymbol(c_sinpi, sinv, sizeof(sinv)));
 }
 
 // ints between the shared-memory areas (two planes) of consecutive teams.  Teams that share a warp must not
@@ -72,9 +113,9 @@ __device__ __forceinline__ const SvtB200InvTxfmItem& inv_part(const SvtB200TrioI
 template <class I> __device__ __forceinline__ const auto& shape_part(const I& i) { return fwd_part(i); }
 
 // the forward's last steps on one coefficient: final shift, then the scaling of 2:1 rectangles
-template <int RECT>
-__device__ __forceinline__ int32_t fwd_out(int32_t v, const TxCfg& cfg) {
-    v = round_shift_arr(v, -cfg.f_s2);
+template <int RECT, int F_S2>
+__device__ __forceinline__ int32_t fwd_out(int32_t v) {
+    v = round_shift_arr(v, -F_S2);
     if constexpr (RECT == 1 || RECT == -1) v = round_shift64((long long)v * kNewSqrt2, 12);
     return v;
 }
@@ -87,16 +128,17 @@ __device__ __forceinline__ int32_t inv_in(int32_t v, int row_clamp) {
 
 // A 1-D pass.  In the 32- and 64-point classes (one block per CTA of 2 * TEAM threads) 32- and 64-point vectors run split
 // across two lanes, shorter ones one per thread.  FULL64: 64-point vectors run whole on one thread, so that all 64 outputs
-// exist (the forward batch's unpacked items); otherwise the 64-point networks are the packed ones.
-template <int TEAM, int THREADS, bool INV, bool FULL64, int N, int V, int P>
-__device__ __forceinline__ void txfm_pass(int type, int32_t* x, int cos_bit, int clampb, int tid) {
+// exist (the forward batch's unpacked items); otherwise the 64-point networks are the packed ones.  COS_BIT: the pass's
+// cosine bit.
+template <int TEAM, int THREADS, bool INV, bool FULL64, int N, int V, int P, int COS_BIT>
+__device__ __forceinline__ void txfm_pass(int type, int32_t* x, int clampb, int tid) {
     if constexpr (TEAM >= 32 && N == 32) {
         static_assert(THREADS == 2 * TEAM, "a lane pair per vector");
-        return txfm_pass_split<32, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
+        return txfm_pass_split<32, THREADS, INV, COS_BIT>(type, x, V, P, clampb, tid);
     } else if constexpr (TEAM >= 64 && N == 64 && !FULL64) {
-        return txfm_pass_split<64, THREADS, INV>(type, x, V, P, cos_bit, clampb, tid);
+        return txfm_pass_split<64, THREADS, INV, COS_BIT>(type, x, V, P, clampb, tid);
     } else {
-        txfm_pass_1d<TEAM, INV, !FULL64>(type, x, N, V, P, cos_bit, clampb, tid);
+        txfm_pass_1d<TEAM, INV, !FULL64, COS_BIT>(type, x, N, V, P, clampb, tid);
     }
 }
 
@@ -191,10 +233,15 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
     constexpr int  Wp = W > 32 ? 32 : W, Hp = H > 32 ? 32 : H;  // 64-point dimensions are packed (inv_transforms.c:2567-2686)
     constexpr int  PW = W + 1, PH = H + 1;  // odd pitches: a plane holds the block as [r * PW + c] or as [c * PH + r]
     constexpr int  VP = kRowWord<W, PIX>, VR = kRowWord<W, int16_t>, VC = kCoefWord;
+    // the size's cosine bits and stage shifts are constants; the flips and the 1-D kernel types come with the type
+    constexpr int  F_CBC = kTxSizeCfg[SZ].f_cbc, F_CBR = kTxSizeCfg[SZ].f_cbr;
+    constexpr int  F_S0 = kTxSizeCfg[SZ].f_s0, F_S1 = kTxSizeCfg[SZ].f_s1, F_S2 = kTxSizeCfg[SZ].f_s2;
+    constexpr int  I_S0 = kTxSizeCfg[SZ].i_s0, I_S1 = kTxSizeCfg[SZ].i_s1;
     const auto&    fi  = fwd_part(item);
     const TxCfg    cfg = c_txcfg[SZ][shape_part(item).tx_type];
+    // 1-byte pixels are 8-bit ones: there the bit depth, and every clamp and range derived from it, is a constant too
     int            bd  = 0;
-    if constexpr (INV) bd = inv_part(item).bd;
+    if constexpr (INV) bd = std::is_same_v<PIX, uint8_t> ? 8 : inv_part(item).bd;
     if constexpr (FWD) {  // ---- forward transform (transforms.c:2286-2318) ----
         const size_t sstride = fi.src_stride;
         // load, optional up/down flip, pre-shift
@@ -211,7 +258,7 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
                     ld_word<decltype(vec)::value>(sp + rr * sstride + c, s);
                     ld_word<decltype(vec)::value>(pp + rr * pstride + c, p);
 #pragma unroll
-                    for (int j = 0; j < VP; j++) A[r * PW + c + j] = round_shift_arr((int32_t)s[j] - (int32_t)p[j], -cfg.f_s0);
+                    for (int j = 0; j < VP; j++) A[r * PW + c + j] = round_shift_arr((int32_t)s[j] - (int32_t)p[j], -F_S0);
                 });
             });
         }
@@ -223,23 +270,23 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
                     int16_t   s[VR];
                     ld_word<decltype(vec)::value>(src + rr * sstride + c, s);
 #pragma unroll
-                    for (int j = 0; j < VR; j++) A[r * PW + c + j] = round_shift_arr((int32_t)s[j], -cfg.f_s0);
+                    for (int j = 0; j < VR; j++) A[r * PW + c + j] = round_shift_arr((int32_t)s[j], -F_S0);
                 });
             });
         }
         team_sync<TEAM, SOLO>();
         // columns: vector v = column v (Chain: rows >= Hp of the result are not needed)
-        txfm_pass<TEAM, THREADS, false, !INV, H, W, PW>(cfg.f_tc, A, cfg.f_cbc, 0, tid);
+        txfm_pass<TEAM, THREADS, false, !INV, H, W, PW, F_CBC>(cfg.f_tc, A, 0, tid);
         team_sync<TEAM, SOLO>();
         // round-shift, optional left/right flip, hand over transposed (element = column); Chain: only the Hp rows that
         // survive the packing
         constexpr int Hk = INV ? Hp : H;
         for_words<W, Hk, 1, MOVERS>(tid, [&](int r, int c) {
             const int cc = cfg.f_lr ? (W - 1 - c) : c;
-            B[cc * PH + r] = round_shift_arr(A[r * PW + c], -cfg.f_s1);
+            B[cc * PH + r] = round_shift_arr(A[r * PW + c], -F_S1);
         });
         team_sync<TEAM, SOLO>();
-        txfm_pass<TEAM, THREADS, false, !INV, W, Hk, PH>(cfg.f_tr, B, cfg.f_cbr, 0, tid);  // rows: vector v = row v
+        txfm_pass<TEAM, THREADS, false, !INV, W, Hk, PH, F_CBR>(cfg.f_tr, B, 0, tid);  // rows: vector v = row v
         team_sync<TEAM, SOLO>();
     }
     if constexpr (!INV) {  // ---- Forward: the coefficients out ----
@@ -254,7 +301,7 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
                 int32_t v[VC];
 #pragma unroll
                 for (int j = 0; j < VC; j++) {
-                    v[j] = fwd_out<RECT>(B[(c + j) * PH + r], cfg);
+                    v[j] = fwd_out<RECT, F_S2>(B[(c + j) * PH + r]);
                     // N2 / N4 (av1_tranform_two_d_core_N2_c / _N4_c, transforms.c:5202, 6769): the top-left half / quarter
                     // of every dimension, identical to the full transform's values there, zero everywhere else
                     if (part_shift && (r >= keep_h || c + j >= keep_w)) v[j] = 0;
@@ -308,7 +355,7 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
                     }
 #pragma unroll
                     for (int j = 0; j < VC; j++) {
-                        const int32_t v = fwd_out<RECT>(B[(c + j) * PH + r], cfg);
+                        const int32_t v = fwd_out<RECT, F_S2>(B[(c + j) * PH + r]);
                         quant_coef<MODE, QM>(k, v, rc + j != 0, QM ? wt[j] : 0, QM ? iwt[j] : 0, q[j], dq[j]);
                         if (q[j]) eob = max(eob, (int)pos[j] + 1);
                         A[(c + j) * PH + r] = inv_in<RECT>(dq[j], row_clamp);
@@ -382,14 +429,14 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
             const int col_clamp = (bd + 6) > 16 ? (bd + 6) : 16;
             const int opt_row = bd == 8 ? 16 : (bd == 10 ? 18 : 20);  // svt_av1_gen_inv_stage_range
             const int opt_col = bd == 12 ? 18 : 16;
-            txfm_pass<TEAM, THREADS, true, false, W, Hp, PH>(cfg.i_tr, A, cfg.i_cbr, opt_row, tid);  // rows >= Hp are zero and stay zero
+            txfm_pass<TEAM, THREADS, true, false, W, Hp, PH, kInvCosBit>(cfg.i_tr, A, opt_row, tid);  // rows >= Hp are zero and stay zero
             team_sync<TEAM, SOLO>();
             for_words<W, H, 1, MOVERS>(tid, [&](int r, int c) {
                 const int cs = cfg.i_lr ? (W - 1 - c) : c;
-                B[r * PW + c] = clamp_bits(round_shift_arr(A[cs * PH + r], -cfg.i_s0), col_clamp);
+                B[r * PW + c] = clamp_bits(round_shift_arr(A[cs * PH + r], -I_S0), col_clamp);
             });
             team_sync<TEAM, SOLO>();
-            txfm_pass<TEAM, THREADS, true, false, H, W, PW>(cfg.i_tc, B, cfg.i_cbc, opt_col, tid);
+            txfm_pass<TEAM, THREADS, true, false, H, W, PW, kInvCosBit>(cfg.i_tc, B, opt_col, tid);
             team_sync<TEAM, SOLO>();
             const long long int_max = (1ll << (7 + bd)) - 1 + (914ll << (bd - 7));  // check_range, inv_transforms.c:2401
             const int       pix_max = (1 << bd) - 1;
@@ -400,7 +447,7 @@ __device__ __forceinline__ void txfm_block(const TxfmPtrs<PIX>& g, const typenam
                     ld_word<decltype(vec_c)::value>(pr + r * pstride + c, p);
 #pragma unroll
                     for (int j = 0; j < VP; j++) {
-                        long long t = (long long)round_shift_arr(B[rs * PW + c + j], -cfg.i_s1);
+                        long long t = (long long)round_shift_arr(B[rs * PW + c + j], -I_S1);
                         t           = t < -int_max - 1 ? -int_max - 1 : (t > int_max ? int_max : t);
                         int v       = (int)p[j] + (int)t;
                         p[j]        = (PIX)(v < 0 ? 0 : (v > pix_max ? pix_max : v));
@@ -431,7 +478,8 @@ __device__ __forceinline__ void dispatch_size(std::integer_sequence<int, SZ...>,
 // CTAs per SM that the register allocation of a class must leave room for: what the class's kernels held before their
 // bodies were specialised by size (168 / 96 / 64 / 64 / 64 registers).  The calls of a step run concurrently on several
 // streams, so a CTA that takes more of an SM's register file keeps other kernels' CTAs off that SM; left free, ptxas
-// gives the specialised bodies up to 235 registers and the step is slower even where the class's own kernel is faster.
+// gives the specialised bodies up to 208 registers and the step is slower even where the class's own kernel is faster.
+// Tighter bounds spill heavily (the 64-point class at 4 CTAs per SM: over 1 KB of spill stores).
 template <int TEAM> constexpr int class_min_ctas() { return TEAM == 64 ? 3 : (TEAM == 32 ? 10 : (TEAM == 16 ? 8 : 4)); }
 
 template <class M, int TEAM, int THREADS, typename PIX>

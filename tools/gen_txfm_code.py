@@ -10,6 +10,10 @@ the 32 outputs the packed coefficient layout keeps (dead nodes dropped), IDCT64_
 32..63 are zero (zero operands folded: half_btf with one zero operand is a single product).  Arithmetic is the reference's: 32-bit wrapping add/sub, half_btf with
 32-bit wrapping products summed in 64 bits (Source/Lib/Codec/inv_transforms.h:264).
 
+Every function is a template on the cosine bit: `cosv` is a TxCosv<cos_bit> (txfm_tables.cuh), the cosine table of
+that bit as a compile-time value, so each weight `cosv[k]` and each rounding shift of half_btf folds to an immediate
+and no weight occupies a register.
+
 Lane splits of the 32- and 64-point DCTs (the ones the fused kernel runs: FDCT32, FDCT64_lo32, IDCT32, IDCT64_in32):
 the network's values after some stage fall into two groups whose cones share nothing but the inputs (which every
 lane reads from shared memory).  split_plan() finds them by slicing the graph: it takes the largest stage count
@@ -103,7 +107,8 @@ def emit(tag, n, stages, name=None, live_out=None, zero_in=None):
             body.append("    const int32_t %s = %s;" % (nm, expr))
             new[i] = nm
         cur = new
-    out.append("__device__ __forceinline__ void txg_%s(int32_t (&x)[%d], const int32_t* __restrict__ cosv, const int cos_bit, const int clampb) {" % (name, n))
+    out.append("template <int cos_bit>")
+    out.append("__device__ __forceinline__ void txg_%s(int32_t (&x)[%d], TxCosv<cos_bit> cosv, const int clampb) {" % (name, n))
     out.append("    (void)clampb;")
     for w in sorted(weights):
         out.append("    const int32_t c%d = cosv[%d];" % (w, w))
@@ -177,15 +182,15 @@ def emit_split(n, stages, name, live_out=None, zero_in=None):
         out.append("")
     mask = {fn: "0x%016xull" % sum(1 << i for i in live) for fn, _, live in fns}
     tail = cut < len(stages)
-    sig = "(int32_t (&x)[%d], const int32_t* __restrict__ cosv, const int cos_bit, const int clampb)" % n
+    sig = "(int32_t (&x)[%d], TxCosv<cos_bit> cosv, const int clampb)" % n
     out.append("struct TxgSplit_%s {" % name)
     out.append("    static constexpr bool kTail = %s;" % ("true" if tail else "false"))
     for k in range(2):
         out.append("    static constexpr unsigned long long kMid%d = %s, kOut%d = %s;" %
                    (k, mask["%s_g%d" % (name, k)], k, mask["%s_%s%d" % (name, "t" if tail else "g", k)]))
     for part, letter in (("mid", "g"), ("tail", "t")) if tail else (("mid", "g"),):
-        out.append("    template <int G> static __device__ __forceinline__ void %s%s {" % (part, sig))
-        out.append("        if constexpr (G == 0) txg_%s_%s0(x, cosv, cos_bit, clampb); else txg_%s_%s1(x, cosv, cos_bit, clampb);" %
+        out.append("    template <int G, int cos_bit> static __device__ __forceinline__ void %s%s {" % (part, sig))
+        out.append("        if constexpr (G == 0) txg_%s_%s0(x, cosv, clampb); else txg_%s_%s1(x, cosv, clampb);" %
                    (name, letter, name, letter))
         out.append("    }")
     out.append("};")
