@@ -28,18 +28,18 @@ lib = _ct.CDLL(LIB_PATH)
 EXPORTS_PATH = _os.path.join(_PKG_DIR, "exports.txt")
 
 
-def header_symbols():
-    """Names of all functions declared in include/svt_b200.h, by preprocessing it (needs gcc: build / test time only)."""
-    import subprocess as _sp
-    txt = _sp.run(["gcc", "-E", "-P", HEADER_PATH], capture_output=True, text=True, check=True).stdout
-    return sorted(set(_re.findall(r"\b(svt_b200_\w+)\s*\(", txt)))
+def prototypes():
+    """The C ABI's functions as [(name, return type, [parameter types])], sorted by name: exports.txt, one prototype
+    per line, written from the header when the library is built (__graft_entry__.build_cuda) and committed, so that
+    importing needs neither gcc nor the header."""
+    with open(EXPORTS_PATH) as f:
+        protos = [_re.fullmatch(r"(.+) (svt_b200_\w+)\((.*)\)", x.strip()).groups() for x in f if x.strip()]
+    return [(name, ret, params.split(", ") if params else []) for ret, name, params in protos]
 
 
 def declared_symbols():
-    """The C ABI's function names: exports.txt, written from the header when the library is built
-    (__graft_entry__.build_cuda) and committed, so that importing needs neither gcc nor the header."""
-    with open(EXPORTS_PATH) as f:
-        return sorted(x.strip() for x in f if x.strip())
+    """The C ABI's function names (exports.txt)."""
+    return [name for name, _, _ in prototypes()]
 
 
 def check_exports():

@@ -1,7 +1,9 @@
 """The C ABI's data layout (include/svt_b200.h), described once: one ctypes.Structure per `typedef struct SvtB200*`, named
 after the C type without `SvtB200`, with the header's fields in the header's order (natural alignment, pointers as
-c_void_p); the numpy dtypes of the T2 work items derived from those; the reference's enumerator values and the plane
-geometry of the ME pyramid.  tests/test_host_logic.py checks every field of every class against the compiled header.
+c_void_p); the numpy dtypes of the T2 work items derived from those; the ctypes type of every C type the header's function
+prototypes use (ctype); the reference's enumerator values and the plane geometry of the ME pyramid.
+tests/test_host_logic.py checks every field of every class against the compiled header, tests/test_abi.py the scalar
+types against the C compiler.
 No library is loaded here -- the module is shared by the product's host mirror (dsp.py), the synthetic workload
 (workload.py) and, loaded stand-alone, by the CPU checkers of the tests and bench.py's CPU reference arm, which must not
 map libsvtav1_b200.so."""
@@ -248,3 +250,26 @@ class PaStatsControls(ct.Structure):
 
 class PaStatsResults(ct.Structure):  # device pointers
     _fields_ = _same(ct.c_void_p, "variance", "pic_avg_variance", "histogram", "average_intensity", "avg_luma")
+
+
+# ---- function signatures --------------------------------------------------------------------------------------------
+C_SCALARS = {"int8_t": ct.c_int8, "uint8_t": ct.c_uint8, "int16_t": ct.c_int16, "uint16_t": ct.c_uint16, "int32_t": ct.c_int32,
+             "uint32_t": ct.c_uint32, "int64_t": ct.c_int64, "uint64_t": ct.c_uint64, "int": ct.c_int, "size_t": ct.c_size_t,
+             "intptr_t": ct.c_ssize_t, "ptrdiff_t": ct.c_ssize_t, "unsigned long long": ct.c_ulonglong}
+
+
+def ctype(c_type, returned=False):
+    """The ctypes type of a normalised C type of the prototypes in exports.txt: void is None, a scalar is its C_SCALARS
+    entry, a SvtB200X passed by value is X above.  Any pointer is c_void_p, except a returned char* (a string): the header
+    cannot tell a host struct from a device item array, and device pointers arrive as integers, so a struct is passed as
+    ct.byref(x) or a ctypes array."""
+    if c_type == "void":
+        return None
+    if "*" in c_type:
+        return ct.c_char_p if returned and c_type == "char*" else ct.c_void_p
+    if c_type in C_SCALARS:
+        return C_SCALARS[c_type]
+    by_value = globals().get(c_type[len("SvtB200"):]) if c_type.startswith("SvtB200") else None
+    if isinstance(by_value, type) and issubclass(by_value, ct.Structure):
+        return by_value
+    raise TypeError("C type %r of include/svt_b200.h has no ctypes counterpart in layout.ctype" % c_type)
