@@ -15,11 +15,13 @@
 // segment of one block (luma: a processed 8-pixel row of an 8x8, chroma: a 4-pixel row of a 4x4 in Cb and the
 // same row in Cr), so the tap offsets of the block's direction and the per-strength constants are built once per
 // segment, not per pixel.  The search evaluates two pixels per step (luma: neighbours, chroma: one per plane).  A
-// pixel's 12 taps are fetched once per direction, as signed differences and magnitudes packed two per
-// register, and shared by all candidate strengths; the filter sum is separable into a primary and a
+// pixel's 12 taps are fetched once per direction, as magnitudes packed two per register with their signs folded
+// into the dot-product weights, and shared by all candidate strengths; the filter sum is separable into a primary and a
 // secondary half, each evaluated once per distinct strength value with native packed 16-bit min/max/add
-// and 2-way dot-product instructions.  The search sums a segment's distortion moments in registers (up
-// to kGChunk strengths at a time), combines the few segments of a block with shuffles and stores them once
+// and 2-way dot-product instructions.  What each candidate strength adds per pixel (rounding, clamp, moments) runs
+// on both pixels of a step at once, in packed 16-bit halves, with the clamp bounds and the pixels' part of the
+// rounding formed once per pixel; at 8 bit the luma moments are IDP.4A byte products.  The search sums a segment's
+// distortion moments in registers (up to kGChunk strengths at a time), combines the few segments of a block with shuffles and stores them once
 // per (block, strength); the source's moments and those of strength code 0 (the unfiltered block) are not
 // recomputed per strength.  The luma distortion's double-precision formula is evaluated with
 // round-to-nearest intrinsics in the reference's operand order (FMA contraction is disabled for the whole
@@ -105,14 +107,21 @@ __device__ int cdef_find_dir_dev(const T* img, int stride, int* var, int coeff_s
 
 // Taps of one pixel along direction `dir` (cdef.c:262-302), reduced to what every candidate strength
 // shares, two taps per 32-bit register (16-bit halves; every value fits: pixels <= 4095, CDEF_VERY_LARGE =
-// 0x7f7f, |differences| <= 0x7f7f): the signed differences tap - x, their magnitudes, and the min / max over
-// the taps that are inside the picture.  Pairs: 0 = primary k=0 (+,-), 1 = primary k=1, 2..3 = secondary
-// k=0, 4..5 = secondary k=1.  The packed min/max/add instructions used (VIMNMX.16x2, VIADD.16x2) are native.
+// 0x7f7f, |differences| <= 0x7f7f): the magnitudes |tap - x|, the dp2a weights of the taps with the sign of
+// tap - x folded in, and the min / max over the taps that are inside the picture.  Pairs: 0 = primary k=0 (+,-),
+// 1 = primary k=1, 2..3 = secondary k=0, 4..5 = secondary k=1.  The packed min/max/add instructions used
+// (VIMNMX.16x2, VIADD.16x2, VIADDMNMX.16x2) are native.
 struct CdefTaps {
-    uint32_t d[6];   // signed differences
     uint32_t ad[6];  // |differences|
-    int      mn, mx;
+    uint32_t wp[2];  // signed dp2a weights of pairs 0-1 (bytes 0-1: pair 0, 2-3: pair 1): [0] weights 4, 2; [1] 3, 3
+    uint32_t w23;    // signed dp2a weights of pairs 2-3 (2 each)
+    uint32_t w45;    // signed dp2a weights of pairs 4-5 (1 each)
+    uint32_t mn2;    // min over the pixel and its taps, per half (CDEF_VERY_LARGE never wins)
+    uint32_t mx2;    // max over the pixel and its taps, per half, each value plus kMxBias (mod 2^16)
 };
+// The maximum over the taps is taken over the halves plus kMxBias (mod 2^16), which maps CDEF_VERY_LARGE to 0 and
+// keeps pixels (<= 4095) in order above it: the sentinel is never the maximum.
+constexpr uint32_t kMxBias = 0x10000u - kVeryLarge;
 // element offsets of the six tap pairs along direction `dir` in a tile of pitch s (pair order as above)
 __device__ __forceinline__ void cdef_tap_offsets(int dir, int s, int (&o)[6]) {
     const int d2 = (dir + 2) & 7, d6 = (dir + 6) & 7;
@@ -123,55 +132,94 @@ __device__ __forceinline__ void cdef_tap_offsets(int dir, int s, int (&o)[6]) {
         o[3 + 2 * k] = c_cdef_dir[d6][k][0] * s + c_cdef_dir[d6][k][1];
     }
 }
+// one byte per 16-bit half of a and b: 0xff where that half is negative (PRMT with sign replication)
+__device__ __forceinline__ uint32_t cdef_sign_bytes(uint32_t a, uint32_t b) {
+    uint32_t r;
+    asm("prmt.b32 %0, %1, %2, 0xFDB9;" : "=r"(r) : "r"(a), "r"(b));
+    return r;
+}
+// weights w (bytes) where the sign byte is 0, -w (bytes nw) where it is 0xff
+__device__ __forceinline__ uint32_t cdef_signed_weights(uint32_t sign, uint32_t w, uint32_t nw) { return (w & ~sign) | (nw & sign); }
 __device__ __forceinline__ void cdef_load_taps(const uint16_t* in, const int (&o)[6], int x, CdefTaps& T) {
-    // CDEF_VERY_LARGE marks "outside the picture": never the maximum.  The maximum is taken over the halves
-    // plus kMxBias (mod 2^16), which maps CDEF_VERY_LARGE to 0 and keeps pixels (<= 4095) in order above it.
-    constexpr uint32_t kMxBias = 0x10000u - kVeryLarge;
     const uint32_t xx = (uint32_t)x * 0x10001u, nxx = __vneg2(xx);
-    uint32_t       mx2 = __vadd2(xx, kMxBias * 0x10001u), mn2 = xx;
+    uint32_t       mx2 = __vadd2(xx, kMxBias * 0x10001u), mn2 = xx, d[6];
 #pragma unroll
     for (int pair = 0; pair < 6; pair++) {
         const uint32_t p = (uint32_t)in[o[pair]] | ((uint32_t)in[-o[pair]] << 16);
-        T.d[pair]  = __vadd2(p, nxx);
+        d[pair]    = __vadd2(p, nxx);
         T.ad[pair] = __vmaxu2(p, xx) - __vminu2(p, xx);  // halves are >= 0: no borrow between them
         mx2 = __vmaxu2(mx2, __vadd2(p, kMxBias * 0x10001u));
         mn2 = __vminu2(mn2, p);
     }
-    T.mn = (int)min(mn2 & 0xffffu, mn2 >> 16);
-    T.mx = (int)max(mx2 & 0xffffu, mx2 >> 16) - (int)kMxBias;
+    const uint32_t sp = cdef_sign_bytes(d[0], d[1]), s23 = cdef_sign_bytes(d[2], d[3]), s45 = cdef_sign_bytes(d[4], d[5]);
+    T.wp[0] = cdef_signed_weights(sp, 0x02020404u, 0xfefefcfcu);
+    T.wp[1] = cdef_signed_weights(sp, 0x03030303u, 0xfdfdfdfdu);
+    T.w23   = cdef_signed_weights(s23, 0x02020202u, 0xfefefefeu);
+    T.w45   = cdef_signed_weights(s45, 0x01010101u, 0xffffffffu);
+    T.mn2 = mn2;
+    T.mx2 = mx2;
 }
-// What constrain() (cdef.c:85-93) needs of a strength t at a damping: the threshold in both halves, the shift
-// max(0, damping - msb(t)), the mask that keeps the shifted high half out of the low one, and the dp2a
-// weights of the two primary pairs (byte pair 0-1: k = 0, 2-3: k = 1; cdef_pri_taps[(t >> coeff_shift) & 1]).
-// t = 0 gives a zero threshold, which constrains every tap to zero.
+// What constrain() (cdef.c:85-93) needs of a strength t at a damping: the threshold plus one in both halves, the
+// shift max(0, damping - msb(t)), the mask that keeps the shifted high half out of the low one, and which primary
+// weights apply (cdef_pri_taps[(t >> coeff_shift) & 1], CdefTaps::wp).  t = 0 gives a zero threshold, which
+// constrains every tap to zero.
 __device__ __forceinline__ uint4 cdef_strength_consts(int t, int damping, int coeff_shift) {
     const int sh = max(0, damping - msb32((uint32_t)t));
-    return make_uint4((uint32_t)t * 0x10001u, (uint32_t)sh, (0xffffu >> sh) * 0x10001u,
-                      ((t >> coeff_shift) & 1) ? 0x03030303u : 0x02020404u);
+    return make_uint4((uint32_t)(t + 1) * 0x10001u, (uint32_t)sh, (0xffffu >> sh) * 0x10001u, (uint32_t)((t >> coeff_shift) & 1));
 }
-// constrain() of the two taps of a pair: sign(d) * min(|d|, max(0, thr - (|d| >> shift))) = clamp(d, -m, m)
-// with m = thr - min(|d| >> shift, thr), as two signed 16-bit halves.
+// |constrain()| of the two taps of a pair: min(|d|, max(0, thr - (|d| >> shift))) = max(min(thr - t1, |d|), 0) with
+// t1 = |d| >> shift, one VIADDMNMX: ~t1 = -t1 - 1 comes with the mask, and c.x = thr + 1.  The sign of d is in the
+// weights the magnitude is multiplied by.
 __device__ __forceinline__ uint32_t cdef_constrain2(const CdefTaps& T, int pair, const uint4& c) {
-    const uint32_t t1 = (T.ad[pair] >> c.y) & c.z;
-    const uint32_t m  = c.x - __vminu2(t1, c.x);
-    return __vmins2(__vmaxs2(T.d[pair], __vneg2(m)), m);
+    const uint32_t nt1 = ~((T.ad[pair] >> c.y) & c.z);
+    return __viaddmin_s16x2_relu(c.x, nt1, T.ad[pair]);
 }
 // The sum splits into a primary part (4 taps, depends on the primary strength only) and a secondary part
 // (8 taps, depends on the secondary strength only): candidate strengths that share one of the two share
 // that half of the work.  The reference accumulates in int16; |sum| <= 2*(4+2)*240 + 4*(2+1)*64 for 12-bit
-// content, so the int32 sum is the same number.  Two constrained secondary taps (|v| <= 64 each) add
-// without overflow in a 16-bit half.
+// content, so the int32 sum is the same number.
 __device__ __forceinline__ int cdef_primary_sum(const CdefTaps& T, const uint4& c) {
-    return __dp2a_hi((int)cdef_constrain2(T, 1, c), (int)c.w, __dp2a_lo((int)cdef_constrain2(T, 0, c), (int)c.w, 0));
+    const int w = (int)(c.w ? T.wp[1] : T.wp[0]);
+    return __dp2a_hi((int)cdef_constrain2(T, 1, c), w, __dp2a_lo((int)cdef_constrain2(T, 0, c), w, 0));
 }
 __device__ __forceinline__ int cdef_secondary_sum(const CdefTaps& T, const uint4& c) {
-    const uint32_t w2 = __vadd2(cdef_constrain2(T, 2, c), cdef_constrain2(T, 3, c));
-    const uint32_t w1 = __vadd2(cdef_constrain2(T, 4, c), cdef_constrain2(T, 5, c));
-    return __dp2a_lo((int)w2, 0x0202, __dp2a_lo((int)w1, 0x0101, 0));
+    const int s = __dp2a_hi((int)cdef_constrain2(T, 3, c), (int)T.w23, __dp2a_lo((int)cdef_constrain2(T, 2, c), (int)T.w23, 0));
+    return __dp2a_hi((int)cdef_constrain2(T, 5, c), (int)T.w45, __dp2a_lo((int)cdef_constrain2(T, 4, c), (int)T.w45, s));
 }
 __device__ __forceinline__ int cdef_finish_px(const CdefTaps& T, int x, int sum) {
+    const int mn = (int)min(T.mn2 & 0xffffu, T.mn2 >> 16), mx = (int)max(T.mx2 & 0xffffu, T.mx2 >> 16) - (int)kMxBias;
     const int y = x + ((8 + sum - (sum < 0)) >> 4);
-    return y < T.mn ? T.mn : (y > T.mx ? T.mx : y);
+    return y < mn ? mn : (y > mx ? mx : y);
+}
+
+// The finish of two pixels at once, pixel A in the low 16-bit halves and pixel B in the high ones.  Every value is
+// kept >= 0 in its half by offsets: a filtered pixel is y + kYOff (y + round(sum) may lie below 0 before the clamp),
+// and a filter sum arrives as sum + kSumOff.  With u = sum + 0x8007, bit 15 of u is set iff sum >= -7, and
+// (u + that bit) >> 4 = ((8 + sum - (sum < 0)) >> 4) + 0x800: the two agree for sum >= 0 and sum < -7, and both
+// roundings give 0 for -7 <= sum < 0.  |sum| <= 3648 (cdef_primary_sum), so no half leaves [0, 2^16).
+constexpr uint32_t kYOff2   = 0x08000800u;  // 0x800 in both halves
+constexpr uint32_t kSumOff2 = 0x80078007u;
+struct CdefPx2 {
+    uint32_t x;       // the two pixels; at 8 bit 16 x (which fits its half), so it is added before the shift
+    uint32_t mn, mx;  // the clamp bounds plus kYOff
+};
+template <typename PIX>
+__device__ __forceinline__ CdefPx2 cdef_px2(const CdefTaps& A, const CdefTaps& B, int xa, int xb) {
+    CdefPx2 P;
+    const uint32_t x2 = (uint32_t)xa | ((uint32_t)xb << 16);
+    P.x  = sizeof(PIX) == 1 ? x2 << 4 : x2;
+    P.mn = __vminu2(__byte_perm(A.mn2, B.mn2, 0x5410), __byte_perm(A.mn2, B.mn2, 0x7632)) + kYOff2;
+    P.mx = __vadd2(__vmaxu2(__byte_perm(A.mx2, B.mx2, 0x5410), __byte_perm(A.mx2, B.mx2, 0x7632)), ((0x800u - kMxBias) & 0xffffu) * 0x10001u);
+    return P;
+}
+// both halves of one filter sum per pixel (sum_a, sum_b: int32 as cdef_primary_sum / cdef_secondary_sum give them)
+__device__ __forceinline__ uint32_t cdef_pack2(int sum_a, int sum_b) { return __byte_perm((uint32_t)sum_a, (uint32_t)sum_b, 0x5410); }
+// the two filtered pixels plus kYOff from u = the packed filter sums plus kSumOff2
+template <typename PIX>
+__device__ __forceinline__ uint32_t cdef_finish2(const CdefPx2& P, uint32_t u) {
+    const uint32_t t = (u >> 15) & 0x00010001u;
+    const uint32_t w = sizeof(PIX) == 1 ? ((u + t + P.x) >> 4) & 0x0fff0fffu : (((u + t) >> 4) & 0x0fff0fffu) + P.x;
+    return __vminu2(__vmaxu2(w, P.mn), P.mx);
 }
 // one filtered pixel; `in` points at the pixel, s = tile pitch
 __device__ __forceinline__ int cdef_filter_px(const uint16_t* in, int s, int pri_strength, int sec_strength, int dir,
@@ -296,7 +344,7 @@ __global__ void search_one_dual_kernel(const unsigned long long* mse0, const uns
 // T2: per-filter-block search (all planes, all candidate strengths) and frame apply
 // ------------------------------------------------------------------------------------------------
 constexpr int kT2Threads = 128;  // threads of a search / apply CTA
-constexpr int kGChunk    = 8;    // candidate strengths whose moments a search thread keeps in registers at once
+constexpr int kGChunk    = 6;    // candidate strengths whose moments a search thread keeps in registers at once (every preset lists 6)
 constexpr int kTPC       = 48;   // chroma tile pitch in uint16 (32 + 2*8, rows 16-B aligned)
 constexpr int kTileC     = (32 + 6) * kTPC;  // one chroma tile; the Cr tile follows the Cb tile
 static_assert(2 * kTileC <= kTileRows * kTP, "both chroma tiles fit where the luma tile goes");
@@ -399,12 +447,34 @@ cdef_dir_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, uint8_t
     var_out[o] = var;
 }
 
+// Phase split of the search (tools/profile_cdef.py): built with B200_CDEF_PHASES=1, thread 0 of every CTA adds the
+// clock64() cycles between consecutive stamps to g_cdef_phase[item][phase] (item 0 = luma, 1 = chroma; phases: table,
+// block list, staging, segment pass 0, pass 1, shuffle combine and source moments, wait for the other segments,
+// distortion warps), and [item][8] counts the items.  Off in the library as shipped: the stamps compile to nothing.
+#ifndef B200_CDEF_PHASES
+#define B200_CDEF_PHASES 0
+#endif
+constexpr int kCdefPhases = 8;
+#if B200_CDEF_PHASES
+__device__ unsigned long long g_cdef_phase[2][kCdefPhases + 1];
+#endif
+__device__ __forceinline__ void cdef_phase(int item, int k, long long& t) {
+#if B200_CDEF_PHASES
+    if (threadIdx.x == 0) {
+        const long long now = clock64();
+        if (k >= 0) atomicAdd(&g_cdef_phase[item][k], (unsigned long long)(now - t));
+        t = now;
+    }
+#endif
+}
+
 // One chunk of candidate strengths (CTA-uniform description) as the search's threads see it.
 struct CdefChunk {
     int      sv[kGChunk];  // strength codes, -1 = not tested (also past the end of the list)
     unsigned todo[2];      // pass 0: taps along the block's direction (a primary part, or code 0); pass 1: along direction 0
     unsigned pri_new;      // pass-0 strengths whose primary code differs from the previous one with a primary part
     unsigned secs[2];      // per pass: bit c set when secondary code c (1..3) occurs
+    unsigned zero;         // strength code 0 (the unfiltered block)
 };
 
 // Moments of one row segment for every strength of `todo`, the taps along one direction.  Luma (BS = 8 pixels at
@@ -419,7 +489,7 @@ __device__ __forceinline__ void cdef_segment_pass(const uint16_t* in, const uint
                                                   const int (&off)[6], const CdefChunk& C, int pass, const int (&tadj)[kGChunk],
                                                   const uint4* tab, int cs, unsigned (&a0)[kGChunk], unsigned (&a1)[kGChunk],
                                                   unsigned (&a2)[kGChunk]) {
-    const unsigned todo = C.todo[pass], pnew = pass ? 0u : C.pri_new, secs = C.secs[pass];
+    const unsigned todo = C.todo[pass], pnew = pass ? 0u : C.pri_new, secs = C.secs[pass], zero = C.zero;
     constexpr int STEP = BS == 8 ? 2 : 1;
 #pragma unroll 1
     for (int j = 0; j < BS; j += STEP) {
@@ -433,46 +503,53 @@ __device__ __forceinline__ void cdef_segment_pass(const uint16_t* in, const uint
             o[k] = BS == 8 ? o_row[j + k] : (k ? o_row2[j] : o_row[j]);
             cdef_load_taps(px[k], off, x[k], T[k]);
         }
-        int s1[2] = {0, 0}, s2[2] = {0, 0}, s3[2] = {0, 0};  // secondary halves of codes 1, 2, 3 (strengths 1, 2, 4 << cs)
+        // what depends on the two pixels alone: the clamp bounds, the pixels in the rounding's form, and the source
+        // operands of the moments (8-bit luma: both source bytes for IDP.4A; chroma: both sources plus kYOff)
+        const CdefPx2  P  = cdef_px2<PIX>(T[0], T[1], x[0], x[1]);
+        const uint32_t x0 = ((uint32_t)x[0] | ((uint32_t)x[1] << 16)) + kYOff2;  // code 0: the pixels themselves
+        const uint32_t ob = BS == 8 ? (sizeof(PIX) == 1 ? o[0] | (o[1] << 8) : 0u) : (o[0] | (o[1] << 16)) + kYOff2;
+        // secondary sums of codes 1, 2, 3 (strengths 1, 2, 4 << cs), packed, plus kSumOff2
+        uint32_t s1 = kSumOff2, s2 = kSumOff2, s3 = kSumOff2;
         if (secs & 2) {
             const uint4 c = tab[1 << cs];
-#pragma unroll
-            for (int k = 0; k < 2; k++) s1[k] = cdef_secondary_sum(T[k], c);
+            s1 = __vadd2(cdef_pack2(cdef_secondary_sum(T[0], c), cdef_secondary_sum(T[1], c)), kSumOff2);
         }
         if (secs & 4) {
             const uint4 c = tab[2 << cs];
-#pragma unroll
-            for (int k = 0; k < 2; k++) s2[k] = cdef_secondary_sum(T[k], c);
+            s2 = __vadd2(cdef_pack2(cdef_secondary_sum(T[0], c), cdef_secondary_sum(T[1], c)), kSumOff2);
         }
         if (secs & 8) {
             const uint4 c = tab[4 << cs];
-#pragma unroll
-            for (int k = 0; k < 2; k++) s3[k] = cdef_secondary_sum(T[k], c);
+            s3 = __vadd2(cdef_pack2(cdef_secondary_sum(T[0], c), cdef_secondary_sum(T[1], c)), kSumOff2);
         }
-        int psum[2] = {0, 0};
+        uint32_t psum = 0;  // packed primary sums of the current primary strength
 #pragma unroll
         for (int gi = 0; gi < kGChunk; gi++) {
             if (!((todo >> gi) & 1)) continue;  // CTA-uniform
             if ((pnew >> gi) & 1) {
                 const uint4 c = tab[tadj[gi]];
-#pragma unroll
-                for (int k = 0; k < 2; k++) psum[k] = cdef_primary_sum(T[k], c);
+                psum = cdef_pack2(cdef_primary_sum(T[0], c), cdef_primary_sum(T[1], c));
             }
-            const int sc = C.sv[gi] & 3;
-#pragma unroll
-            for (int k = 0; k < 2; k++) {
-                const int ssum = sc == 1 ? s1[k] : (sc == 2 ? s2[k] : (sc == 3 ? s3[k] : 0));
-                // code 0 leaves the pixel unchanged (sum = 0, and x lies inside [min, max] of its own neighbourhood)
-                const unsigned y = C.sv[gi] == 0 ? (unsigned)x[k] : (unsigned)cdef_finish_px(T[k], x[k], psum[k] + ssum);
-                if (BS == 8) {
-                    a0[gi] += y;
-                    a1[gi] += y * y;
-                    a2[gi] += y * o[k];
-                } else {
-                    const int e = (int)o[k] - (int)y;
-                    if (k == 0) a0[gi] += (unsigned)(e * e);
-                    else a1[gi] += (unsigned)(e * e);
-                }
+            const int      sc = C.sv[gi] & 3;
+            const uint32_t ss = sc & 2 ? (sc & 1 ? s3 : s2) : (sc & 1 ? s1 : kSumOff2);
+            // code 0 leaves the pixel unchanged (sum = 0, and x lies inside [min, max] of its own neighbourhood)
+            const uint32_t y = (zero >> gi) & 1 ? x0 : cdef_finish2<PIX>(P, __vadd2(psum, ss));  // both pixels plus kYOff
+            if (BS == 8 && sizeof(PIX) == 1) {
+                // pixels <= 255: the low byte of each half is the pixel (kYOff has none), and every product fits IDP.4A
+                const uint32_t yb = __byte_perm(y, 0, 0x4420);
+                a0[gi] = __dp4a(yb, 0x01010101u, a0[gi]);
+                a1[gi] = __dp4a(yb, yb, a1[gi]);
+                a2[gi] = __dp4a(yb, ob, a2[gi]);
+            } else if (BS == 8) {
+                const uint32_t yy = y - kYOff2, ya = yy & 0xffffu, yb = yy >> 16;
+                a0[gi] = __dp2a_lo(yy, 0x0101u, a0[gi]);
+                a1[gi] += ya * ya + yb * yb;
+                a2[gi] += ya * o[0] + yb * o[1];
+            } else {
+                const uint32_t e = __vsub2(ob, y);  // Cb and Cr errors, signed halves
+                const int      ea = (int)(int16_t)(e & 0xffffu), eb = (int)e >> 16;
+                a0[gi] += (unsigned)(ea * ea);
+                a1[gi] += (unsigned)(eb * eb);
             }
         }
     }
@@ -487,16 +564,15 @@ template <int BS, typename PIX>
 __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4* tab, const PIX* src, const PIX* src2, int sstride,
                                                const int* strengths, int n_strengths, int count, int subs, int cs, const uint8_t* s_list,
                                                const uint8_t* s_dir, const int* s_var, unsigned (*s_mom)[3][64], unsigned (*s_src)[64],
-                                               unsigned long long* mse_fb) {
-    constexpr int TP = BS == 8 ? kTP : kTPC;
+                                               unsigned long long* mse_fb, long long& ph_t) {
+    constexpr int TP = BS == 8 ? kTP : kTPC, IT = BS == 8 ? 0 : 1;
     const int R = BS / subs, nseg = count * R;  // processed rows per block (a power of two: R divides 32)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int g0 = 0; g0 < n_strengths; g0 += kGChunk) {
         const int ng = min(kGChunk, n_strengths - g0);
         CdefChunk C;
-        C.todo[0] = C.todo[1] = C.pri_new = C.secs[0] = C.secs[1] = 0;
-        unsigned zero = 0;
-        int      last_pri = -1;
+        C.todo[0] = C.todo[1] = C.pri_new = C.secs[0] = C.secs[1] = C.zero = 0;
+        int last_pri = -1;
 #pragma unroll
         for (int gi = 0; gi < kGChunk; gi++) {
             const int sv = gi < ng ? strengths[g0 + gi] : -1;
@@ -512,12 +588,12 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
                 C.todo[1] |= 1u << gi;
                 C.secs[1] |= 1u << sc;
             } else {
-                zero |= 1u << gi;
+                C.zero |= 1u << gi;
             }
         }
         // code 0 needs no taps: it joins a pass that runs anyway
-        if (C.todo[0] || !C.todo[1]) C.todo[0] |= zero;
-        else C.todo[1] |= zero;
+        if (C.todo[0] || !C.todo[1]) C.todo[0] |= C.zero;
+        else C.todo[1] |= C.zero;
         const unsigned tested = C.todo[0] | C.todo[1];
         for (int s = threadIdx.x; s < ((nseg + 31) & ~31); s += kT2Threads) {  // whole warps stay in the loop (shuffles)
             const bool live = s < nseg;
@@ -541,10 +617,12 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
                 cdef_tap_offsets(s_dir[b], TP, off);
                 cdef_segment_pass<BS, PIX>(in, in + kTileC, o_row, o_row2, off, C, 0, tadj, tab, cs, a0, a1, a2);
             }
+            cdef_phase(IT, 3, ph_t);
             if (C.todo[1]) {
                 cdef_tap_offsets(0, TP, off);
                 cdef_segment_pass<BS, PIX>(in, in + kTileC, o_row, o_row2, off, C, 1, tadj, tab, cs, a0, a1, a2);
             }
+            cdef_phase(IT, 4, ph_t);
             const bool lead = live && r == 0;
 #pragma unroll
             for (int gi = 0; gi < kGChunk; gi++) {
@@ -577,8 +655,10 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
                     s_src[1][bi] = so2;
                 }
             }
+            cdef_phase(IT, 5, ph_t);
         }
         __syncthreads();
+        cdef_phase(IT, 6, ph_t);
         // per strength: the blocks' distortions, summed by one warp
         for (int gi = warp; gi < ng; gi += kT2Threads / 32) {
             const int          sv = strengths[g0 + gi];
@@ -605,6 +685,7 @@ __device__ __forceinline__ void cdef_search_fb(const uint16_t* tile, const uint4
             }
         }
         __syncthreads();  // s_mom is reused by the next chunk
+        cdef_phase(IT, 7, ph_t);
     }
 }
 
@@ -617,9 +698,13 @@ __device__ __forceinline__ bool cdef_item(int work, int nfb, int& fb) {
 }
 
 // Strength search: one CTA per filter block and luma, and one per filter block and both chroma planes.  Every
-// mse[plane][fb][g] is written once.
+// mse[plane][fb][g] is written once.  Six CTAs per SM hold the segment loop without a spill (80 registers); the bound
+// can be set at build time to measure others (DESIGN §5, §7).
+#ifndef CDEF_SEARCH_CTAS
+#define CDEF_SEARCH_CTAS 6
+#endif
 template <typename PIX>
-__global__ void __launch_bounds__(kT2Threads, 5)
+__global__ void __launch_bounds__(kT2Threads, CDEF_SEARCH_CTAS)
 cdef_search_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, const int* __restrict__ strengths_y,
                    const int* __restrict__ strengths_uv, int n_strengths, unsigned long long* __restrict__ mse /*[2][nfb][n_strengths]*/,
                    const uint8_t* __restrict__ dir_in /*[nfb][64]*/, const int* __restrict__ var_in /*[nfb][64]*/) {
@@ -635,18 +720,25 @@ cdef_search_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, cons
     const int cs = f.bit_depth > 8 ? f.bit_depth - 8 : 0;
     const int w8 = (f.width + 7) >> 3, h8 = (f.height + 7) >> 3;
     int tab_damping = -1;
+    long long ph_t = 0;
     for (int work = blockIdx.x; work < nfb * 2; work += gridDim.x) {
         int        fb;
         const bool chroma = cdef_item(work, nfb, fb);
         const int  fbr = fb / nhfb, fbc = fb - fbr * nhfb;
         const int  damping = f.damping + cs - chroma;
+        cdef_phase(chroma, -1, ph_t);
         __syncthreads();
         if (damping != tab_damping) {  // CTA-uniform; cdef_fb_list's barrier publishes the table
             // strengths reach (15 << 4) = 240 (primary, 12-bit), adjusted ones no more, secondary 4 << 4
             for (int i = threadIdx.x; i < 256; i += kT2Threads) s_tab[i] = cdef_strength_consts(i, damping, cs);
             tab_damping = damping;
         }
+        cdef_phase(chroma, 0, ph_t);
+#if B200_CDEF_PHASES
+        if (threadIdx.x == 0) atomicAdd(&g_cdef_phase[chroma][kCdefPhases], 1ull);
+#endif
         const int count = cdef_fb_list(skip8x8, dir_in, var_in, fb, fbr, fbc, w8, h8, s_list, s_dir, s_var, s_ballot);
+        cdef_phase(chroma, 1, ph_t);
         unsigned long long* mse_fb = mse + (size_t)(chroma * nfb + fb) * n_strengths;
         if (count == 0) {
             for (int g = threadIdx.x; g < n_strengths; g += blockDim.x) mse_fb[g] = 0;
@@ -656,17 +748,19 @@ cdef_search_kernel(SvtB200CdefFrame f, const uint8_t* __restrict__ skip8x8, cons
             const int hsz = min(64, f.width - fbc * 64), vsz = min(64, f.height - fbr * 64);
             const PIX* rec = (const PIX*)f.recon_y;
             stage_cdef_tiles<PIX, 1>(tile, rec, rec, f.recon_stride_y, fbr, fbc, nvfb, nhfb, vsz, hsz);  // ends with a barrier
+            cdef_phase(0, 2, ph_t);
             const PIX* src_fb = (const PIX*)f.src_y + (size_t)fbr * 64 * f.src_stride_y + fbc * 64;
             const int  subs = min(f.subsampling_factor, 4);  // cdef_process.c:243-248
             cdef_search_fb<8, PIX>(tile, s_tab, src_fb, src_fb, f.src_stride_y, strengths_y, n_strengths, count, subs, cs, s_list, s_dir,
-                                   s_var, s_mom, s_src, mse_fb);
+                                   s_var, s_mom, s_src, mse_fb, ph_t);
         } else {
             const int hsz = min(32, (f.width >> 1) - fbc * 32), vsz = min(32, (f.height >> 1) - fbr * 32);
             stage_cdef_tiles<PIX, 2>(tile, (const PIX*)f.recon_cb, (const PIX*)f.recon_cr, f.recon_stride_c, fbr, fbc, nvfb, nhfb, vsz, hsz);
+            cdef_phase(1, 2, ph_t);
             const size_t o = (size_t)fbr * 32 * f.src_stride_c + fbc * 32;
             const int subs = min(f.subsampling_factor, 1);  // 4:2:0 chroma = BLOCK_4X4
             cdef_search_fb<4, PIX>(tile, s_tab, (const PIX*)f.src_cb + o, (const PIX*)f.src_cr + o, f.src_stride_c, strengths_uv, n_strengths,
-                                   count, subs, cs, s_list, s_dir, s_var, s_mom, s_src, mse_fb);
+                                   count, subs, cs, s_list, s_dir, s_var, s_mom, s_src, mse_fb, ph_t);
         }
     }
 }
@@ -903,6 +997,16 @@ extern "C" uint64_t svt_b200_search_one_dual(int* lev0, int* lev1, int nb_streng
 }
 
 // ---- T2 ------------------------------------------------------------------------------------------
+#if B200_CDEF_PHASES
+// the search's phase split since the last read (see cdef_phase), then zeroed; only in a B200_CDEF_PHASES build
+extern "C" SVT_B200_API int svt_b200_cdef_phases_read(unsigned long long* out /*[2][kCdefPhases + 1]*/) {
+    static const unsigned long long zeros[2][kCdefPhases + 1] = {};
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, g_cdef_phase, sizeof(zeros)) != cudaSuccess ||
+        cudaMemcpyToSymbol(g_cdef_phase, zeros, sizeof(zeros)) != cudaSuccess)
+        return -1;
+    return 0;
+}
+#endif
 extern "C" int svt_b200_cdef_search_frame_dev(const SvtB200CdefFrame* frame, const uint8_t* d_skip8x8, const int* d_strengths_y,
                                               const int* d_strengths_uv, int n_strengths, uint64_t* d_mse, uint8_t* d_dir,
                                               int32_t* d_var, void* stream) {
