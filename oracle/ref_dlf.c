@@ -1,5 +1,5 @@
-/* oracle/ref_dlf.c -- TEST / BASELINE INFRASTRUCTURE, compiled into oracle/_ref/libsvtav1_dlf.so (oracle/dlf.mk), which takes
- * every reference symbol from oracle/_ref/libsvtav1_ref.so.
+/* oracle/ref_dlf.c -- TEST / BASELINE INFRASTRUCTURE, compiled into oracle/_ref/libsvtav1_dlf.so (`make -C oracle dlf`),
+ * which takes every reference symbol from oracle/_ref/libsvtav1_ref.so.
  *
  * Deblocking of one picture through the reference's OWN loop filter: svt_av1_loop_filter_init + svt_av1_loop_filter_frame
  * (deblocking_filter.c:36, :625) run on the caller's planes, with a minimal SequenceControlSet / PictureParentControlSet /

@@ -1,5 +1,5 @@
 /* oracle/ref_dlf_search.c -- TEST / BASELINE INFRASTRUCTURE, compiled into oracle/_ref/libsvtav1_dlf_search.so
- * (oracle/dlf_search.mk), which takes every reference symbol from oracle/_ref/libsvtav1_ref.so.
+ * (`make -C oracle dlf_search`), which takes every reference symbol from oracle/_ref/libsvtav1_ref.so.
  *
  * The deblocking filter-level search through the reference's own functions, on the picture ref_dlf.c builds from flat
  * mode-info records and a RefDlfCfg (ref_dlf.c is included, so both checkers construct the picture the same way):

@@ -1,5 +1,5 @@
-/* oracle/ref_pa_stats.c -- TEST / BASELINE INFRASTRUCTURE, compiled into oracle/_ref/libsvtav1_pa_stats.so (oracle/pa_stats.mk),
- * which takes every reference symbol from oracle/_ref/libsvtav1_ref.so.
+/* oracle/ref_pa_stats.c -- TEST / BASELINE INFRASTRUCTURE, compiled into oracle/_ref/libsvtav1_pa_stats.so
+ * (`make -C oracle pa_stats`), which takes every reference symbol from oracle/_ref/libsvtav1_ref.so.
  *
  * The picture-analysis statistics through the reference's OWN svt_aom_gathering_picture_statistics
  * (pic_analysis_process.c:1559): block variances, region histograms, average intensities, avg_luma and pic_avg_variance

@@ -7,6 +7,8 @@ import sys
 
 import pytest
 
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 

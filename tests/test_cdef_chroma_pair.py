@@ -15,6 +15,7 @@ import pytest
 
 import cdef_helpers as ch
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 pytestmark = pytest.mark.gpu
 

@@ -3,12 +3,12 @@ against the reference's own svt_av1_loop_filter_frame (oracle/ref_dlf.c), and on
 rests on -- two whole-plane passes (every vertical edge, then every horizontal edge) give the reference's superblock-order
 result, and the small AV1 tables of dlf_tables.h are the reference's."""
 import ctypes as ct
-import os
 
 import numpy as np
 import pytest
 
 from helpers import rng
+from oracle_libs import dlf as dlfc, refc  # noqa: F401  (fixtures; refc overrides conftest.py's in this module)
 
 LPF_TAPS = (4, 6, 8, 14)
 
@@ -25,19 +25,6 @@ class RefDlfCfg(ct.Structure):  # oracle/ref_dlf.c
                [("ref_deltas", ct.c_int32 * 8), ("mode_deltas", ct.c_int32 * 2), ("segmentation_enabled", ct.c_int32),
                 ("seg_lf_enabled", (ct.c_int32 * 4) * 8), ("seg_lf_data", (ct.c_int32 * 4) * 8)] + \
                [(n, ct.c_int32) for n in ("mi_rows", "mi_cols", "mi_stride", "reserved")]
-
-
-DLF_LIB = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libsvtav1_dlf.so")
-
-
-@pytest.fixture(scope="module")
-def dlfc(refc):
-    """oracle/_ref/libsvtav1_dlf.so (oracle/dlf.mk): oracle/ref_dlf.c and the deblocking glue, on top of the reference
-    objects refc has loaded and initialised"""
-    if not os.path.exists(DLF_LIB):
-        pytest.fail("oracle/_ref/libsvtav1_dlf.so is missing: build it with `python __graft_entry__.py --oracle` where the "
-                    "reference sources are available")
-    return ct.CDLL(DLF_LIB)
 
 
 def _layout():

@@ -4,25 +4,13 @@ hill-climb (search_filter_level, deblocking_filter.c:886), run over a table of o
 chooses what its own sequential search (svt_av1_pick_filter_level, LPF_PICK_FROM_FULL_IMAGE: ref_dlf_pick) chooses, with
 the same zero_filt_sse / best_filt_sse.  On the CPU with the reference's table, on the GPU with the device's."""
 import ctypes as ct
-import os
 
 import numpy as np
 import pytest
 
 from helpers import rng
+from oracle_libs import dlf_search as dlfc  # noqa: F401  (a fixture)
 from test_deblock import FORMATS, SIZES, _layout, make_cfg, make_mode_info, make_planes
-
-DLF_SEARCH_LIB = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "libsvtav1_dlf_search.so")
-
-
-@pytest.fixture(scope="module")
-def dlfc(refc):
-    """oracle/_ref/libsvtav1_dlf_search.so (oracle/dlf_search.mk): oracle/ref_dlf_search.c and the deblocking glue, on top
-    of the reference objects refc has loaded and initialised"""
-    if not os.path.exists(DLF_SEARCH_LIB):
-        pytest.fail("oracle/_ref/libsvtav1_dlf_search.so is missing: build it with `python __graft_entry__.py --oracle` where "
-                    "the reference sources are available")
-    return ct.CDLL(DLF_SEARCH_LIB)
 
 ONLY_4X4, TX_MODE_LARGEST, TX_MODE_SELECT = 0, 1, 2
 KEY_FRAME, INTER_FRAME = 0, 1

@@ -11,6 +11,7 @@ import pytest
 import me_helpers as mh
 import rest_helpers as rh
 from helpers import rng, sad_loop_call
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 pytestmark = pytest.mark.gpu
 

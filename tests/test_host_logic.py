@@ -10,6 +10,8 @@ import tempfile
 import numpy as np
 import pytest
 
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 

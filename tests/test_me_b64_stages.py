@@ -8,6 +8,7 @@ import me_helpers as mh
 import test_me_b64 as base
 from helpers import rng
 from oracle import support as sp
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 pytestmark = pytest.mark.gpu
 

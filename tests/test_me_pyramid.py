@@ -10,6 +10,7 @@ import pytest
 import me_helpers as mh
 from helpers import rng
 from oracle import support as sp
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 pytestmark = pytest.mark.gpu
 

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from helpers import rng, sad_loop_call, sad_pattern
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 BLOCKS = [(16, 16), (32, 32), (64, 64), (16, 8), (64, 32), (24, 24), (31, 7), (4, 4), (48, 64), (5, 11), (128, 128)]
 AREAS = [(8, 3), (16, 31), (15, 6), (48, 40), (64, 25)]

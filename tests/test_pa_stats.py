@@ -5,16 +5,14 @@ pre-filled with a sentinel so that the entries it does not write are known.  The
 integration glue (svt_b200_pa_controls_from_scs) and stores the device results back into a pcs through it
 (svt_b200_pa_store_results)."""
 import ctypes as ct
-import os
 
 import numpy as np
 import pytest
 
 from helpers import rng
 from oracle import support as sp
+from oracle_libs import pa_stats, refc  # noqa: F401  (fixtures; refc overrides conftest.py's in this module)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PA_LIB = os.path.join(ROOT, "oracle", "_ref", "libsvtav1_pa_stats.so")
 layout = sp.layout
 
 # sentinels (bit patterns) of the outputs: an entry that still holds one after a call was not written
@@ -31,16 +29,12 @@ class RefPaStatsOut(ct.Structure):
 
 
 @pytest.fixture(scope="module")
-def pa(refc, request):
-    if not os.path.exists(PA_LIB):
-        pytest.fail("oracle/_ref/libsvtav1_pa_stats.so is missing: build it with `python __graft_entry__.py --oracle` where the "
-                    "reference sources are available")
-    lib = ct.CDLL(PA_LIB)
-    lib.ref_pa_stats.argtypes = [ct.c_void_p] * 4
-    lib.ref_pa_stats.restype = ct.c_int
-    lib.ref_pa_stats_store.argtypes = [ct.c_void_p, ct.c_void_p, ct.c_void_p, ct.c_uint16, ct.c_void_p, ct.c_void_p, ct.c_uint64, ct.c_void_p]
-    lib.ref_pa_stats_store.restype = ct.c_int
-    return lib
+def pa(pa_stats):
+    pa_stats.ref_pa_stats.argtypes = [ct.c_void_p] * 4
+    pa_stats.ref_pa_stats.restype = ct.c_int
+    pa_stats.ref_pa_stats_store.argtypes = [ct.c_void_p, ct.c_void_p, ct.c_void_p, ct.c_uint16, ct.c_void_p, ct.c_void_p, ct.c_uint64, ct.c_void_p]
+    pa_stats.ref_pa_stats_store.restype = ct.c_int
+    return pa_stats
 
 
 def cfg(var=1, sub=1, var8=1, hist=1, scd=0, regions=(4, 4)):

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 pytestmark = pytest.mark.gpu
 

@@ -12,6 +12,7 @@ import rest_helpers as rh
 import test_restoration_frame as trf
 from helpers import rng
 from oracle.support import layout
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 from test_restoration_frame import PAD, _plane, _units
 from test_restoration_paths import LEGAL_HI, LEGAL_LO, _reference, _run, _taps, _wiener_units
 

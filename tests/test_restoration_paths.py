@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 from test_restoration_frame import PAD, _plane, _units
 
 pytestmark = pytest.mark.gpu

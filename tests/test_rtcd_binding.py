@@ -21,18 +21,20 @@ import sys
 import numpy as np
 import pytest
 
+from oracle_libs import enc, refc  # noqa: F401  (fixtures; refc overrides conftest.py's in this module)
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ENC_LIB = os.path.join(ROOT, "oracle", "_ref", "libsvtav1_enc.so")
 
 _ENCODE = r'''
 import ctypes as ct, hashlib, json, os, sys, time
 import numpy as np
 sys.path.insert(0, %(root)r)
+import oracle
 from oracle.frame_ref import load_workload_module
 W = load_workload_module()
-lib = ct.CDLL(%(lib)r)
+lib = oracle.load("enc")
 lib.ref_encode.restype = ct.c_int64
 lib.ref_encode.argtypes = [ct.c_void_p] + [ct.c_int] * 8 + [ct.c_void_p, ct.c_int64, ct.c_void_p]
 w, h, n, bd, preset, crf, lp = %(w)d, %(h)d, %(n)d, %(bd)d, %(preset)d, %(crf)d, %(lp)d
@@ -63,23 +65,16 @@ def _encode(b200_on, groups=None, **kw):
         env["SVT_B200_DEVICE"] = "0"
         if groups is not None:
             env["SVT_B200_RTCD_GROUPS"] = str(groups)
-    code = _ENCODE % dict(kw, root=ROOT, lib=ENC_LIB, b200=os.path.join(ROOT, "svt-av1-psy_b200", "libsvtav1_b200.so"))
+    code = _ENCODE % dict(kw, root=ROOT, b200=os.path.join(ROOT, "svt-av1-psy_b200", "libsvtav1_b200.so"))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=1500)
     assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-3000:])
     line = [x for x in r.stdout.splitlines() if x.startswith("RESULT ")][-1]
     return json.loads(line[7:])
 
 
-def _need_lib():
-    if not os.path.exists(ENC_LIB):
-        pytest.fail("oracle/_ref/libsvtav1_enc.so is missing: `make -C oracle enc` where /root/reference exists")
-
-
-def test_install_rtcd_binds_the_reference_pointers(b200):
+def test_install_rtcd_binds_the_reference_pointers(b200, enc):
     """every T1 entry point lands on the reference's own global function pointers"""
     import ctypes as ct
-    _need_lib()
-    enc = ct.CDLL(ENC_LIB)
     enc.ref_set_tier.restype = ct.c_int
     enc.ref_set_tier(0)  # svt_aom_setup_*_rtcd_internal(0): everything = *_c
     before = ct.c_void_p.in_dll(enc, "svt_sad_loop_kernel").value
@@ -96,15 +91,13 @@ def test_install_rtcd_binds_the_reference_pointers(b200):
 
 
 @pytest.mark.parametrize("name", ["frame_384x256", "frame_384x256_b10_m6"])
-def test_reference_process_loops_with_b200_pointers_match_c_goldens(b200, name):
+def test_reference_process_loops_with_b200_pointers_match_c_goldens(b200, enc, name):
     """oracle/ref_driver.c's frame step = the reference's own loops around the dispatched pointers (svt_cdef_filter_fb,
     svt_aom_inv_transform_recon*, svt_aom_copy_sb8_16, svt_av1_compute_stats*, wiener convolve ...).  Run with the H100
     T1 functions installed, every output must hash to the committed C-tier fixture."""
     import ctypes as ct
     from oracle.frame_ref import RefFrame, load_workload_module
-    _need_lib()
     g = json.load(open(os.path.join(ROOT, "tests", "golden", name + ".json")))
-    enc = ct.CDLL(ENC_LIB)
     enc.ref_set_tier.restype = ct.c_int
     enc.ref_set_tier(0)
     assert enc.svt_b200_install_rtcd(0) == 0
@@ -125,13 +118,11 @@ def test_reference_process_loops_with_b200_pointers_match_c_goldens(b200, name):
     enc.ref_set_tier(0)
 
 
-def test_lr_filter_unit_with_b200_pointers(b200, refc):
+def test_lr_filter_unit_with_b200_pointers(b200, refc, enc):
     """svt_av1_loop_restoration_filter_unit (restoration.c:1067) -- stripes, saved boundary lines, Wiener and self-guided --
     with the H100 convolve / self-guided functions installed == the same call on the C tier"""
     import ctypes as ct
     from test_oracle_pins import _lr_case  # the fixture generator of the a13 oracle pins
-    _need_lib()
-    enc = ct.CDLL(ENC_LIB)
     enc.ref_set_tier.restype = ct.c_int
     for kind in ("wiener", "sgrproj"):
         res = []
@@ -150,9 +141,9 @@ def test_lr_filter_unit_with_b200_pointers(b200, refc):
 @pytest.mark.parametrize("cfg", [dict(w=640, h=360, n=6, bd=8, preset=12, crf=35, lp=8), dict(w=640, h=360, n=4, bd=8, preset=8, crf=30, lp=8),
                                  dict(w=640, h=360, n=4, bd=10, preset=8, crf=30, lp=1)],
                          ids=["configs0_360p_8bit_M12", "360p_8bit_M8", "360p_10bit_M8_lp1"])
+@pytest.mark.usefixtures("enc")  # the encodes load it in processes of their own
 def test_encoder_bitstream_identical_to_c_path(cfg):
     """SURVEY.md 8(c)(ii): the encoder with the H100 tier installed writes the same bitstream as `--asm c`"""
-    _need_lib()
     c = _encode(False, **cfg)
     g = _encode(True, **cfg)
     assert c["bytes"] > 0 and c["packets"] == cfg["n"], c
@@ -171,11 +162,11 @@ SGR_W, SGR_H, SGR_N = 640, 360, 4
 # reason given above
 @pytest.mark.parametrize("cfg", [dict(w=SGR_W, h=SGR_H, n=SGR_N, bd=8, preset=3, crf=35, lp=8), dict(w=SGR_W, h=SGR_H, n=SGR_N, bd=10, preset=3, crf=35, lp=1)],
                          ids=["8bit_M3", "10bit_M3_lp1"])
+@pytest.mark.usefixtures("enc")  # the encodes load it in processes of their own
 def test_encoder_with_only_sgr_pointers_identical_to_c_path(cfg):
     """with only the self-guided restoration pointers installed (kernel group 128: the filter, apply, both projection
     errors and the projection subspace), the restoration search of a preset-3 encode calls them in its own shapes, and the
     bitstream is the `--asm c` one"""
-    _need_lib()
     c = _encode(False, **cfg)
     g = _encode(True, groups=128, **cfg)
     assert c["bytes"] > 0 and c["packets"] == cfg["n"], c

@@ -26,6 +26,7 @@ import pytest
 
 import rest_helpers as rh
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 from test_restoration_frame import PAD, _plane
 from test_restoration_paths import _reference, _run
 

@@ -8,16 +8,14 @@ import pytest
 
 import rest_helpers as rh
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 from test_oracle_pins import _sgr_inputs
 
 pytestmark = pytest.mark.gpu
 
 
-def test_selfguided_filter_and_projection(b200, oracle):
+def test_selfguided_filter_and_projection(b200, refc):
     r = rng(110)
-    refc = oracle.ref
-    if refc is None:
-        pytest.skip("needs oracle/_ref")
     ppe8 = refc.svt_av1_lowbd_pixel_proj_error_c; ppe8.restype = ct.c_int64
     ppe16 = refc.svt_av1_highbd_pixel_proj_error_c; ppe16.restype = ct.c_int64
     gps = refc.svt_get_proj_subspace_c; gps.restype = None

@@ -18,6 +18,7 @@ import pytest
 
 import chain_helpers as ch
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 from txfm_helpers import TX_H, TX_W, ref_fwd_partial
 
 BAD_ARG = -4  # SVT_B200_ERR_BAD_ARG
@@ -25,13 +26,11 @@ gpu = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
-def ref(oracle):
-    """the reference's C kernels with every host CPU on the batches; without them the GPU tests fail, never skip"""
-    if oracle.ref is None:
-        pytest.fail("oracle/_ref/libsvtav1_ref.so is missing: build it with `python __graft_entry__.py --oracle`")
-    oracle.ref.ref_set_tier(0)
-    oracle.ref.ref_set_threads(0)
-    return oracle.ref
+def ref(refc):
+    """the reference's C kernels with every host CPU on the batches"""
+    refc.ref_set_tier(0)
+    refc.ref_set_threads(0)
+    return refc
 
 
 @pytest.fixture(scope="module")

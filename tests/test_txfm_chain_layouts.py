@@ -18,6 +18,7 @@ import pytest
 
 import chain_helpers as ch
 from helpers import rng
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 from quant_helpers import tables_for
 from svt_av1_psy_b200.workload import av1_tables
 from txfm_helpers import TX_H, TX_W
@@ -162,12 +163,10 @@ def _assert_reached(case, mixed):
 
 
 @pytest.fixture(scope="module")
-def ref(oracle):
-    if oracle.ref is None:
-        pytest.fail("oracle/_ref/libsvtav1_ref.so is missing: build it with `python __graft_entry__.py --oracle`")
-    oracle.ref.ref_set_tier(0)
-    oracle.ref.ref_set_threads(0)
-    return oracle.ref
+def ref(refc):
+    refc.ref_set_tier(0)
+    refc.ref_set_threads(0)
+    return refc
 
 
 @pytest.fixture(scope="module")

@@ -11,17 +11,11 @@ import pytest
 
 import rest_helpers as rh
 from helpers import rng
+from oracle_libs import refc as ref  # noqa: F401  (a fixture)
 
 pytestmark = pytest.mark.gpu
 
 PAD = 8  # the reference reads up to 3 pixels beyond the region: a region on the picture edge reads this padding
-
-
-@pytest.fixture(scope="module")
-def ref(oracle):
-    if oracle.ref is None:
-        pytest.fail("oracle/_ref/libsvtav1_ref.so is missing: build it with `python __graft_entry__.py --oracle`")
-    return oracle.ref
 
 
 def _content(r, kind, w, h):

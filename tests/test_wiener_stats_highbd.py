@@ -18,6 +18,7 @@ import pytest
 import rest_helpers as rh
 from helpers import rng
 from oracle.support import layout
+from oracle_libs import refc  # noqa: F401  (a fixture: overrides conftest.py's refc in this module)
 
 gpu = pytest.mark.gpu
 
@@ -263,13 +264,11 @@ def test_cases_reach_every_boundary(bd):
 
 # ---- GPU ---------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def ref(oracle):
-    if oracle.ref is None:
-        pytest.fail("oracle/_ref/libsvtav1_ref.so is missing: build it with `python __graft_entry__.py --oracle`")
-    oracle.ref.ref_set_tier(0)
-    oracle.ref.ref_set_threads(0)
-    oracle.ref.ref_compute_stats_batch_bd.restype = None
-    return oracle.ref
+def ref(refc):
+    refc.ref_set_tier(0)
+    refc.ref_set_threads(0)
+    refc.ref_compute_stats_batch_bd.restype = None
+    return refc
 
 
 @pytest.fixture(scope="module")

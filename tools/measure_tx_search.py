@@ -16,10 +16,12 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import oracle  # noqa: E402
 from oracle.frame_ref import load_workload_module  # noqa: E402
 
 W, H, N, PRESET, CRF = ([int(a) for a in sys.argv[1:6]] + [1920, 1080, 17, 8, 30][len(sys.argv) - 1:])[:5]
-lib = ct.CDLL(os.path.join(ROOT, "oracle", "_ref", "libsvtav1_enc.so"))
+lib = oracle.load("enc")
+assert lib is not None, "libsvtav1_enc.so: " + oracle.BUILD_HINT
 lib.ref_encode.restype = ct.c_int64
 lib.ref_encode.argtypes = [ct.c_void_p] + [ct.c_int] * 8 + [ct.c_void_p, ct.c_int64, ct.c_void_p]
 lib.ref_counters_read.restype = ct.c_int

@@ -9,7 +9,6 @@ once), and prints the card, its power limit and max SM clock in the same run.  W
 it also times the reference's own svt_av1_pick_filter_level (ref_dlf_pick: the whole search, sequential tries of
 whole-plane filter + SSE + restore) once per case on one host core.
 Usage: python tools/profile_dlf_search.py [--calls N] [--no-host]"""
-import ctypes as ct
 import json
 import os
 import subprocess
@@ -21,7 +20,6 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-DLF_LIB = os.path.join(ROOT, "oracle", "_ref", "libsvtav1_dlf_search.so")
 
 
 def main():
@@ -29,10 +27,10 @@ def main():
     import svt_av1_psy_b200 as pkg
     from test_deblock_search import ref_pick, search_case, search_sharpness
     calls = int(sys.argv[sys.argv.index("--calls") + 1]) if "--calls" in sys.argv else 200
-    host = "--no-host" not in sys.argv and os.path.exists(DLF_LIB)
-    if host:
-        import oracle  # noqa: F401  (loads and initialises the reference objects the checker library links to)
-        dlfc = ct.CDLL(DLF_LIB)
+    dlfc = None
+    if "--no-host" not in sys.argv:
+        import oracle
+        dlfc = oracle.load("dlf_search")
     pkg.init(0)
     d = pkg.dsp
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
@@ -83,7 +81,7 @@ def main():
             print(json.dumps({"case": "%dx%d %d-bit" % (w, h, bd), "levels": name, "median_ms": round(med, 4), "calls": calls,
                               "us_per_plane_level": round(1000 * med / (len(levels) * (1 if mask == 1 else 3)), 2),
                               "min_bytes": nbytes, "gbs": round(nbytes / med / 1e6, 1)}))
-        if host:
+        if dlfc is not None:
             t0 = time.perf_counter()
             picked, _, _ = ref_pick(dlfc, cfg, mi, rec, src, ctl)
             print(json.dumps({"case": "%dx%d %d-bit" % (w, h, bd), "host_ref_pick_ms": round(1000 * (time.perf_counter() - t0), 1),

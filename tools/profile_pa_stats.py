@@ -42,9 +42,9 @@ def main():
     from oracle import support as sp
     dsp = pkg.dsp
     pkg.init(0)
-    pa = ct.CDLL(tp.PA_LIB) if os.path.exists(tp.PA_LIB) else None
+    import oracle
+    pa = oracle.load("pa_stats")
     if pa is not None:
-        import oracle  # noqa: F401  (binds the reference's dispatch pointers to the C functions)
         pa.ref_pa_stats.argtypes = [ct.c_void_p] * 4
         pa.ref_pa_stats.restype = ct.c_int
     print("gpu:", gpu_info())
